@@ -13,9 +13,17 @@
 // as two halves of 128 x 32 (S x 16 accumulator registers per thread, 128 for S = 8).
 //   warpgroup 0   TMA producer (one thread): per 64-byte k-block ONE box {64 B, 128 rows, S slices} of A and one
 //                 {64 B, 32 rows, S} of B (cp.async.bulk.tensor.3d, SWIZZLE_64B, mbarrier complete_tx) into a ring
-//   warpgroups 1-2  consumers, rows 0-63 / 64-127 of the tile: per K = 32 step, slice s of A against slices 0..S-1-s of B
-//                 as ONE wgmma with N = 32 (S - s) (B slices adjacent in shared memory, accumulators adjacent in the
-//                 register fragment); then the epilogue: Horner-combine the S accumulators in fp64 (exact int32 -> double
+//   warpgroups 1-2  consumers, rows 0-63 / 64-127 of the tile: per K = 32 step, slice s of A against slices 0..S-1-s of B,
+//                 grouped by PAIRS of diagonals {0,1}, {2,3}, ... (B slices adjacent in shared memory, accumulators
+//                 adjacent in the register fragment): for each group {lo, lo+1} with lo > s - 1 one wgmma with N = 64 (32
+//                 for a last, single diagonal) over B slices lo - s, lo - s + 1.  For odd s diagonal s alone is left: at
+//                 S <= 7 it goes to an extra accumulator (16 registers, folded into diagonal s by an exact int32 add
+//                 before the epilogue), at S = 8 (no registers for 4 extras) the group {s-1, s} runs over a zero B block
+//                 placed in front of B slice 0.  So every wgmma writes a whole group or an extra accumulator: runs that
+//                 partially overlap would make ptxas serialise the chain, one wgmma in flight at a time.  All wgmmas of a
+//                 64-byte k-block are issued in one go (19 per K = 32 step at S = 7, 20 at S = 8) with A from registers
+//                 (ldmatrix from the swizzled stage) for as many slices as the register budget allows, the rest from
+//                 shared memory.  Then the epilogue: Horner-combine the S diagonals in fp64 (exact int32 -> double
 //                 through the 2^52 trick), scale by 2^(e_row + e_col) and add into C (red.global.add.f64: the
 //                 read-modify-write happens in L2, as one correctly rounded addition per element)
 // The slicing kernel (oz_slice_kernel) is O(rows*K) and runs once per panel; in the Cholesky its output is shared by
@@ -40,11 +48,23 @@ constexpr int OZ_THREADS = 384;
 
 template <int S>
 struct OzCfg {
+  // Diagonal schedule (see the header): PAD = zero block in front of B slice 0 (odd A slices use a window starting in it),
+  // otherwise odd diagonals get EXTRA accumulators of their own.  The first RA A slices are read into registers (8 per
+  // slice and k-block), the rest straight from shared memory, so that accumulators + A fragments stay within 192 of the
+  // consumers' 232 registers: S <= 6 all in registers; S = 7: 160 accumulators, slices 0-3 in registers; S = 8 would need
+  // 192 accumulators, so it pads (3 resp. 4 zero products per K = 32 step on top of 28 resp. 36 for S = 7 / 8 padded) and
+  // keeps its 8 slices in registers.
+  static constexpr bool PAD = S > 7;
+  static constexpr int EXTRA = PAD ? 0 : S / 2;
+  static constexpr int ACC = 16 * (S + EXTRA);  // int32 accumulator registers per thread
+  static constexpr int RA = (192 - ACC) / 8 < S ? (192 - ACC) / 8 : S;
   static constexpr int A_SLICE = OZ_BM * OZ_BK;  // 8 KB
   static constexpr int B_SLICE = OZ_HN * OZ_BK;  // 2 KB
   static constexpr int A_BYTES = S * A_SLICE;
+  static constexpr int Z_BYTES = PAD ? B_SLICE : 0;
   static constexpr int B_BYTES = S * B_SLICE;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int TX_BYTES = A_BYTES + B_BYTES;  // what the TMA writes per stage
+  static constexpr int STAGE_BYTES = A_BYTES + Z_BYTES + B_BYTES;
   static constexpr int SMEM_MAX = 226 * 1024;  // 227 KB per CTA minus the static barriers / alignment slack
   static constexpr int STAGES = (SMEM_MAX - 1024) / STAGE_BYTES > 4 ? 4 : (SMEM_MAX - 1024) / STAGE_BYTES;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;
@@ -91,12 +111,38 @@ __device__ __forceinline__ void oz_tma_load_3d(void* dst, const CUtensorMap* map
 __device__ __forceinline__ double oz_i2d(uint32_t x) {
   return __hiloint2double(0x43300000, (int)(x ^ 0x80000000u)) - 4503601774854144.0;  // 2^52 + 2^31
 }
-// One K = 32 step of a consumer warpgroup: A slice SA (64 rows) against B slices 0 .. S-1-SA, accumulators SA .. S-1
+// A slice SA (64 rows) times the N rows of B at b_addr: A from its registers a + 4 SA (SA < RA) or from the stage (a_addr)
+template <int S, int SA, int N>
+__device__ __forceinline__ void oz_wgmma(uint32_t* d, const uint32_t* a, uint32_t a_addr, uint32_t b_addr, uint32_t accumulate) {
+  if constexpr (SA < OzCfg<S>::RA)
+    wgmma_s8_ra<N>(d, a + 4 * SA, wgmma_desc<64>(b_addr), accumulate);
+  else
+    wgmma_s8<N>(d, wgmma_desc<64>(a_addr + SA * OzCfg<S>::A_SLICE), wgmma_desc<64>(b_addr), accumulate);
+}
+// Diagonal group {LO, LO + 1} (or the last, single {S - 1}) of A slice SA: B slices LO - SA .. into accumulators LO ..
+template <int S, int SA, int LO>
+__device__ __forceinline__ void oz_mma_groups(uint32_t* acc, const uint32_t* a, uint32_t a_addr, uint32_t b_addr,
+                                              uint32_t accumulate) {
+  constexpr int W = S - LO < 2 ? S - LO : 2;
+  oz_wgmma<S, SA, OZ_HN * W>(acc + 16 * LO, a, a_addr, b_addr + (LO - SA) * OzCfg<S>::B_SLICE, accumulate);
+  if constexpr (LO + 2 < S) oz_mma_groups<S, SA, LO + 2>(acc, a, a_addr, b_addr, accumulate);
+}
+// One K = 32 step of a consumer warpgroup: A slice SA against B slices 0 .. S-1-SA.  Every wgmma writes a whole diagonal
+// group or an extra accumulator, so no two of them write overlapping, unequal register runs (which makes ptxas serialise
+// the wgmma chain).  The first step of a pass (accumulate = 0) starts with SA = 0, which writes every group.
 template <int S, int SA>
-__device__ __forceinline__ void oz_mma_step(uint32_t* acc, uint32_t a_addr, uint32_t b_addr, uint32_t accumulate) {
-  wgmma_s8<OZ_HN * (S - SA)>(acc + 16 * SA, wgmma_desc<64>(a_addr + SA * OzCfg<S>::A_SLICE), wgmma_desc<64>(b_addr),
-                             accumulate);
-  if constexpr (SA + 1 < S) oz_mma_step<S, SA + 1>(acc, a_addr, b_addr, 1u);
+__device__ __forceinline__ void oz_mma_step(uint32_t* acc, const uint32_t* a, uint32_t a_addr, uint32_t b_addr,
+                                            uint32_t accumulate) {
+  using Cfg = OzCfg<S>;
+  if constexpr (SA & 1) {
+    if constexpr (Cfg::PAD)  // group {SA - 1, SA}: window from the zero block in front of B slice 0
+      oz_wgmma<S, SA, 2 * OZ_HN>(acc + 16 * (SA - 1), a, a_addr, b_addr - Cfg::B_SLICE, 1u);
+    else  // diagonal SA alone, into its extra accumulator
+      oz_wgmma<S, SA, OZ_HN>(acc + 16 * (S + SA / 2), a, a_addr, b_addr, accumulate);
+  }
+  constexpr int LO = (SA + 1) & ~1;  // first group that lies wholly at or above diagonal SA
+  if constexpr (LO < S) oz_mma_groups<S, SA, LO>(acc, a, a_addr, b_addr, SA == 0 ? accumulate : 1u);
+  if constexpr (SA + 1 < S) oz_mma_step<S, SA + 1>(acc, a, a_addr, b_addr, accumulate);
 }
 // tile index -> (tile row, tile column).  Lower mode enumerates only the tiles that touch the lower triangle: row tm holds
 // nc(tm) = min(tiles_n, 2 (tm + 1)) tiles (128 x 64 tiles), so f(r) = r (r + 1) tiles precede row r while r <= tri_rows.
@@ -161,6 +207,13 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     }
     fence_mbar_init();
   }
+  if constexpr (Cfg::PAD) {  // the zero blocks: written once, never touched by the TMA, read by the wgmmas (async proxy)
+    for (int i = threadIdx.x; i < STAGES * Cfg::Z_BYTES / 16; i += OZ_THREADS) {
+      const int st = i / (Cfg::Z_BYTES / 16), j = i % (Cfg::Z_BYTES / 16);
+      reinterpret_cast<uint4*>(smem + st * Cfg::STAGE_BYTES + Cfg::A_BYTES)[j] = make_uint4(0, 0, 0, 0);
+    }
+    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+  }
   __syncthreads();
   const int KB = p.KB;
 
@@ -176,9 +229,9 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
             const int s = g % STAGES, it = g / STAGES;
             if (it > 0) oz_mbar_wait(&empty_bar[s], (it - 1) & 1);
             uint8_t* st = smem + s * Cfg::STAGE_BYTES;
-            mbar_arrive_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
+            mbar_arrive_expect_tx(&full_bar[s], Cfg::TX_BYTES);
             oz_tma_load_3d(st, &mapA, kb * OZ_BK, p.a_row0 + tm * OZ_BM, 0, &full_bar[s]);
-            oz_tma_load_3d(st + Cfg::A_BYTES, &mapB, kb * OZ_BK, p.b_row0 + tn * OZ_BN + h * OZ_HN, 0, &full_bar[s]);
+            oz_tma_load_3d(st + Cfg::A_BYTES + Cfg::Z_BYTES, &mapB, kb * OZ_BK, p.b_row0 + tn * OZ_BN + h * OZ_HN, 0, &full_bar[s]);
           }
         }
       }
@@ -190,28 +243,43 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   const int r_lo = 16 * (tid >> 5) + ((tid & 31) >> 2), c_lo = 2 * (tid & 3);
   // 2^-(12 + 7 (S-1)): weight of the last kept diagonal; Horner runs from diagonal 0 (largest weight) down
   const double w_last = __hiloint2double((1023 - (12 + 7 * (S - 1))) << 20, 0);
-  uint32_t acc[16 * S];
+  // ldmatrix.x4 source of this lane inside an A slice, for the two K = 32 halves of the 64-byte (SWIZZLE_64B) row: matrix
+  // lane / 8 = rows +8 (bit 0) and bytes +16 (bit 1), 16-byte chunk XOR (row / 2) % 4
+  const int lane = tid & 31, a_row = wrow + 16 * (tid >> 5) + (lane & 7) + 8 * ((lane >> 3) & 1);
+  const uint32_t a_off0 = a_row * OZ_BK + ((((lane >> 4) + 0) ^ ((lane >> 1) & 3)) << 4);
+  const uint32_t a_off1 = a_row * OZ_BK + ((((lane >> 4) + 2) ^ ((lane >> 1) & 3)) << 4);
+  uint32_t acc[Cfg::ACC];
   int g = 0;
   for (int t = t_begin; t < t_end; ++t) {
     int tm, tn;
     oz_tile(p, t, tm, tn);
     for (int h = 0; h < 2; ++h) {
-      // ---- main loop: the MMAs of k-block kb run while the previous stage is handed back to the producer ----
+      // ---- main loop: all wgmmas of a k-block in flight at once, A fragments in registers ----
       for (int kb = 0; kb < KB; ++kb, ++g) {
         const int s = g % STAGES, it = g / STAGES;
         oz_mbar_wait(&full_bar[s], it & 1);
-        const uint32_t a0 = smem_u32(smem + s * Cfg::STAGE_BYTES) + wrow * OZ_BK, b0 = smem_u32(smem + s * Cfg::STAGE_BYTES) + Cfg::A_BYTES;
+        const uint32_t st = smem_u32(smem + s * Cfg::STAGE_BYTES), b0 = st + Cfg::A_BYTES + Cfg::Z_BYTES;
+        uint32_t a[2][4 * Cfg::RA];
+#pragma unroll
+        for (int sl = 0; sl < Cfg::RA; ++sl) {
+          ldmatrix_x4(a[0] + 4 * sl, st + sl * Cfg::A_SLICE + a_off0);
+          ldmatrix_x4(a[1] + 4 * sl, st + sl * Cfg::A_SLICE + a_off1);
+        }
         wgmma_fence();
 #pragma unroll
         for (int ks = 0; ks < 2; ++ks)  // wgmma K = 32 int8 = 32 bytes inside the 64-byte swizzle row
-          oz_mma_step<S, 0>(acc, a0 + ks * 32, b0 + ks * 32, (kb > 0 || ks > 0) ? 1u : 0u);
+          oz_mma_step<S, 0>(acc, a[ks], st + wrow * OZ_BK + ks * 32, b0 + ks * 32, (kb > 0 || ks > 0) ? 1u : 0u);
         wgmma_commit();
-        wgmma_wait<1>();
-        if (kb > 0) oz_mbar_arrive(&empty_bar[(g - 1) % STAGES]);
+        wgmma_wait<0>();  // (the A registers are rewritten by the next k-block; the other consumer keeps the tensor cores busy)
+        oz_mbar_arrive(&empty_bar[s]);
       }
-      wgmma_wait<0>();
-      oz_mbar_arrive(&empty_bar[(g - 1) % STAGES]);
       // ---- epilogue: Horner-combine the diagonals in fp64, scale, add into C ----
+      if constexpr (Cfg::EXTRA > 0) {  // fold the extra accumulators into their diagonals (exact int32 sums)
+#pragma unroll
+        for (int d = 1; d < S; d += 2)
+#pragma unroll
+          for (int i = 0; i < 16; ++i) acc[16 * d + i] += acc[16 * (S + d / 2) + i];
+      }
       const int64_t row0 = (int64_t)tm * OZ_BM + wrow + r_lo;
       const int64_t col0 = (int64_t)tn * OZ_BN + h * OZ_HN + c_lo;
 #pragma unroll

@@ -270,8 +270,10 @@ __global__ void __launch_bounds__(KM_THREADS) kernel_matrix_kernel(const KmParam
 //     (<= 128 registers, >= 2 CTAs per SM so one CTA's TMA wait / transpose / barrier hides under the other's arithmetic);
 //   * fp64 exp = 2^(k/64) table (shared memory) x degree-5 polynomial on |r| <= ln2/128 with a two-part Cody-Waite reduction:
 //     11 FP64-pipe operations instead of the ~25 of the library exp (which also handles overflow / NaN paths that a
-//     non-positive argument never takes); relative error < 3e-16 (table entry rounding + 5 Horner steps), i.e. well
-//     inside the 1e-12 parity budget on K (tests/test_gpu_primitives.py compares at rtol 1e-12 against the oracle).
+//     non-positive argument never takes); relative error <= 4.0e-16 (at most 2 ulp; table entry rounding + 5 Horner
+//     steps), i.e. well inside the 1e-12 parity budget on K (tests/test_gpu_primitives.py compares at rtol 1e-12 against
+//     the oracle).  Results below the normal range (x < -708.4) are flushed to 0 where the library exp returns a denormal.
+//     tests/_fexp_model.py restates this function operation for operation; tests/test_kernel_edges.py checks it.
 __device__ __forceinline__ double fast_exp_nonpos(double x, const double* __restrict__ tab) {
   // x <= 0.  k = round(x * 64 / ln2); x = k * ln2/64 + r; exp(x) = 2^(k >> 6) * tab[k & 63] * exp(r)
   const double t = fma(x, 92.332482616893656877, 6755399441055744.0);  // 64 / ln2, 1.5 * 2^52: round-to-nearest in the low bits
@@ -285,8 +287,13 @@ __device__ __forceinline__ double fast_exp_nonpos(double x, const double* __rest
   p = fma(p, r, 1.0);
   p = fma(p, r, 1.0);
   const double v = p * tab[k & 63];
-  const int e = k >> 6;  // <= 0
-  if (e < -1022) return 0.0;  // below the normal range: exp(x) < 2.3e-308 (the library would return a denormal)
+  const int e = k >> 6;
+  // Range check, in the integer pipe: the result is valid for k in [-65408, 0] (k >> 6 >= -1022) with t's high word that
+  // of 1.5 * 2^52 + k (0x4337ffff for k < 0, 0x43380000 for k = 0).  Anything else is an exp(x) below the normal range
+  // (flushed to 0), -inf, an x so negative that k no longer fits the low 32 bits of t (the exponent arithmetic would write
+  // garbage into the sign and exponent bits), or a NaN, which stays a NaN.
+  const int ht = __double2hiint(t);
+  if ((unsigned)k + 65408u > 65408u || ht - (k >> 31) != 0x43380000) return ((ht & 0x7fffffff) > 0x7ff00000) ? t : 0.0;
   return __hiloint2double(__double2hiint(v) + e * 1048576, __double2loint(v));
 }
 

@@ -58,9 +58,12 @@ __device__ __forceinline__ void eval_factor_grad(int kind, T d2, T dot, bool sam
       return;
     }
     case GPK_MATERN12: {
+      // not differentiable at r = 0: coincident points get the subgradient 0, the value autograd gives through the
+      // reference's |x - y| (d = 1) and sqrt(max(d2, 1e-30)) (d > 1)
+      const bool flat = (d == 1) ? !(d2 > T(0)) : !(d2 > T(1e-30));
       T r = (d == 1) ? kb_sqrt<T>(d2) : kb_sqrt<T>(d2 > T(1e-30) ? d2 : T(1e-30));
       val = kb_exp<T>(-r);
-      dval = same_pt ? T(0) : -val / (T(2) * (r > T(1e-300) ? r : T(1e-300)));
+      dval = (same_pt || flat) ? T(0) : -val / (T(2) * r);
       return;
     }
     case GPK_MATERN32: {
@@ -94,19 +97,24 @@ __device__ __forceinline__ void eval_factor_grad(int kind, T d2, T dot, bool sam
   }
 }
 
+// The partial sums of grad_xg take 256 * G * 4 * d words of shared memory.  For wide inputs the launch is split over
+// chunks of dimensions (blockIdx.z = chunk): every chunk evaluates the full distances and kernel values but keeps partial
+// sums only for its dimensions [k0, k0 + dc); chunk 0 alone writes term_sum and diag.
 template <typename T>
-__global__ void __launch_bounds__(KB_THREADS) kernel_matrix_bwd_kernel(const KbParams p) {
+__global__ void __launch_bounds__(KB_THREADS) kernel_matrix_bwd_kernel(const KbParams p, const int dc) {
   const int tile_r = blockIdx.x, b = blockIdx.y;
   const int d = p.d, G = p.desc.n_groups, nt = p.desc.n_terms;
+  const int k0 = blockIdx.z * dc, k1 = min(d, k0 + dc);
+  const bool first = blockIdx.z == 0;
   const int64_t r0 = (int64_t)tile_r * KB_TILE;
   extern __shared__ __align__(16) unsigned char kb_smem[];
   T* xs = reinterpret_cast<T*>(kb_smem);            // [G][64][d]   rows of this CTA
   T* yt = xs + (size_t)G * KB_TILE * d;              // [G][d][65]   current column tile, transposed
-  T* part = yt + (size_t)G * d * (KB_TILE + 1);      // [256 threads][G][4 rows][d + 1]: (sum_j c_ij x_jk ..., sum_j w_ij)
+  T* part = yt + (size_t)G * d * (KB_TILE + 1);      // [256 threads][G][4 rows][dc]: sum_j of d K_ij / d x_ik, k in the chunk
   const T* xg = static_cast<const T*>(p.xg) + (int64_t)b * p.x_bstride;
   const T* Gm = static_cast<const T*>(p.G) + (int64_t)b * p.g_bstride;
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const int pstride = G * 4 * (d + 1);
+  const int pstride = G * 4 * dc;
   T* mypart = part + (size_t)tid * pstride;
   for (int i = 0; i < pstride; ++i) mypart[i] = T(0);
 
@@ -177,39 +185,39 @@ __global__ void __launch_bounds__(KB_THREADS) kernel_matrix_bwd_kernel(const KbP
             const T wgt = gij * ct * others * dval[q];
             const int g = p.desc.fac_group[f0 + q];
             const int kind = p.desc.fac_kind[f0 + q];
-            T* pp = mypart + ((size_t)g * 4 + i) * (d + 1);
+            T* pp = mypart + ((size_t)g * 4 + i) * dc;  // pp[k - k0] for the dimensions k of this chunk
             const T* yc_ = yt + (size_t)g * d * (KB_TILE + 1) + tx + 16 * j;
             if (kind == GPK_LINEAR) {
               // d(dot)/dx_ik = x_jk ; factor 2 for the symmetric counterpart
-              for (int k = 0; k < d; ++k) pp[k] = fma(T(2) * wgt, yc_[(size_t)k * (KB_TILE + 1)], pp[k]);
+              for (int k = k0; k < k1; ++k) pp[k - k0] = fma(T(2) * wgt, yc_[(size_t)k * (KB_TILE + 1)], pp[k - k0]);
             } else {
-              // d(d2)/dx_ik = 2 (x_ik - x_jk) ; factor 2 for the symmetric counterpart:
-              //   grad_ik += 4 wgt x_ik - 4 wgt x_jk  -> keep sum_j wgt in slot d, sum_j wgt x_jk in slot k
-              for (int k = 0; k < d; ++k) pp[k] = fma(T(-4) * wgt, yc_[(size_t)k * (KB_TILE + 1)], pp[k]);
-              pp[d] += T(4) * wgt;
+              // d(d2)/dx_ik = 2 (x_ik - x_jk) ; factor 2 for the symmetric counterpart.  The difference is formed per
+              // pair: Matern-1/2's weight grows like 1/r for near-coincident points, and splitting it into
+              // 4 wgt x_ik - 4 wgt x_jk would cancel catastrophically.
+              const T* xr_ = xs + ((size_t)g * KB_TILE + ty * 4 + i) * d;
+              for (int k = k0; k < k1; ++k)
+                pp[k - k0] = fma(T(4) * wgt, xr_[k] - yc_[(size_t)k * (KB_TILE + 1)], pp[k - k0]);
             }
           }
         }
-        if (same_pt && p.diag) static_cast<T*>(p.diag)[(int64_t)b * p.n + r] = gij;
+        if (first && same_pt && p.diag) static_cast<T*>(p.diag)[(int64_t)b * p.n + r] = gij;
       }
     }
   }
   __syncthreads();
-  // reduce the 16 column-threads of every row and write grad_xg
+  // reduce the 16 column-threads of every row and write this chunk's columns of grad_xg
   T* gout = static_cast<T*>(p.grad_xg) + (int64_t)b * p.x_bstride;
-  for (int idx = tid; idx < G * KB_TILE * d; idx += KB_THREADS) {
-    const int g = idx / (KB_TILE * d), rem = idx - g * KB_TILE * d;
-    const int row = rem / d, k = rem - row * d;
+  const int w = k1 - k0;
+  for (int idx = tid; idx < G * KB_TILE * w; idx += KB_THREADS) {
+    const int g = idx / (KB_TILE * w), rem = idx - g * KB_TILE * w;
+    const int row = rem / w, kk = rem - row * w;
     if (r0 + row >= p.n) continue;
     const int rty = row >> 2, ri = row & 3;
-    T s = T(0), sw = T(0);
-    for (int t16 = 0; t16 < 16; ++t16) {
-      const T* pp = part + (size_t)(rty * 16 + t16) * pstride + ((size_t)g * 4 + ri) * (d + 1);
-      s += pp[k];
-      sw += pp[d];
-    }
-    gout[g * p.xg_gstride + (r0 + row) * d + k] = s + sw * xs[(size_t)g * KB_TILE * d + row * d + k];
+    T s = T(0);
+    for (int t16 = 0; t16 < 16; ++t16) s += part[(size_t)(rty * 16 + t16) * pstride + ((size_t)g * 4 + ri) * dc + kk];
+    gout[g * p.xg_gstride + (r0 + row) * d + k0 + kk] = s;
   }
+  if (!first) return;
   // term sums: block reduction + one atomic per term
   __shared__ T red[8][GPK_MAX_TERMS];
 #pragma unroll
@@ -249,16 +257,22 @@ static int launch_kernel_matrix_bwd(const gpk_kernel_desc* desc, const T* xg, in
   p.grad_xg = grad_xg;
   p.diag = diag;
   const int Gn = desc->n_groups;
-  const size_t smem =
-      ((size_t)Gn * KB_TILE * d + (size_t)Gn * d * (KB_TILE + 1) + (size_t)KB_THREADS * Gn * 4 * (d + 1)) * sizeof(T);
-  if (smem > 200 * 1024) return GPK_ERR_UNSUPPORTED;
+  // input rows + transposed column tile (all d dimensions), then as many dimensions of partial sums as fit
+  constexpr size_t kMaxSmem = 200 * 1024;
+  const size_t rows_bytes = ((size_t)Gn * KB_TILE * d + (size_t)Gn * d * (KB_TILE + 1)) * sizeof(T);
+  const size_t dim_bytes = (size_t)KB_THREADS * Gn * 4 * sizeof(T);
+  if (rows_bytes + dim_bytes > kMaxSmem) return GPK_ERR_UNSUPPORTED;
+  const size_t fit = (kMaxSmem - rows_bytes) / dim_bytes;
+  const int dc = fit < (size_t)d ? (int)fit : d;
+  const int chunks = (d + dc - 1) / dc;
+  const size_t smem = rows_bytes + (size_t)dc * dim_bytes;
   auto kern = kernel_matrix_bwd_kernel<T>;
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return -1000 - (int)e;
   }
-  dim3 grid((unsigned)((n + KB_TILE - 1) / KB_TILE), (unsigned)batch);
-  kern<<<grid, KB_THREADS, smem, (cudaStream_t)stream>>>(p);
+  dim3 grid((unsigned)((n + KB_TILE - 1) / KB_TILE), (unsigned)batch, (unsigned)chunks);
+  kern<<<grid, KB_THREADS, smem, (cudaStream_t)stream>>>(p, dc);
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();
   return 0;

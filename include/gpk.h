@@ -18,6 +18,10 @@
  *     Numerical failure (non-positive pivot) is reported LAPACK-style through the device-side `info` word
  *     (index of the first bad pivot, 1-based; 0 = success) so that no host sync is forced.
  *   - `_f64` / `_f32` suffix = arithmetic type (double / float); everything is computed in that type.
+ *   - The one environment variable the library reads is GPK_NO_LOOKAHEAD, at every gpk_potrf_* call.  When it is set,
+ *     the factorisation enqueues all its work on `stream` instead of factorising the next panel on side streams while
+ *     the trailing update runs, so that CUDA events around a launch time that kernel alone.  It is meant for profiling:
+ *     the factorisation is slower with it.
  */
 #ifndef GPK_H_
 #define GPK_H_

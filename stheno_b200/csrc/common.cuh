@@ -3,6 +3,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <atomic>
+#include <mutex>
+
 #include "../../include/gpk.h"
 
 namespace gpk {
@@ -16,6 +19,26 @@ extern long long g_launch_count;  // defined in util.cu
   } while (0)
 
 #define GPK_COUNT_LAUNCH() (++::gpk::g_launch_count)
+
+// Lets `Kernel` launch with `bytes` of dynamic shared memory on the current device.  CUDA keeps this opt-in per kernel and
+// per device, so the largest size set so far is remembered per device and the driver is called only for a larger
+// request.  Returns 0, -1000 - cudaError, or GPK_ERR_UNSUPPORTED on a device ordinal above 63.
+template <auto Kernel>
+int opt_in_smem(int bytes) {
+  static std::atomic<int> set[64];  // by device ordinal
+  static std::mutex mu;             // never lowers a size another host thread has just set
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return -1000 - (int)e;
+  if (dev >= 64) return GPK_ERR_UNSUPPORTED;
+  if (bytes <= set[dev].load(std::memory_order_acquire)) return 0;
+  std::lock_guard<std::mutex> lock(mu);
+  if (bytes <= set[dev].load(std::memory_order_relaxed)) return 0;
+  e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return -1000 - (int)e;
+  set[dev].store(bytes, std::memory_order_release);
+  return 0;
+}
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));

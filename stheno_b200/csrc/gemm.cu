@@ -1,24 +1,26 @@
 // GEMM  C = beta*C + alpha * A * B^T  (NT: both operands K-contiguous) -- the BLAS-3 engine of the Cholesky
 // trailing update (SYRK, lower tiles only), the panel updates, the recursive TRSM and the posterior covariance.
 //
-// fp64: 128 x 128 x 16 CTA tile, 8 warps (2 x 4), each warp a 64 x 32 tile of DMMA.8x8x4 fragments (fp64 tensor
-//   cores; wgmma has no f64 type).  Operands are staged by a 4-stage cp.async (LDGSTS) pipeline into a
-//   FRAGMENT-MAJOR shared-memory layout: the 16-byte granule holding (row, k = 2j, 2j+1) is stored where lane
-//   (row % 8) * 4 + j of the owning 8-row block reads it, so every fragment load is one conflict-free,
-//   warp-contiguous LDS.128 that feeds TWO DMMAs (the even-k one and the odd-k one -- the k order inside a
-//   k-group of 8 is permuted identically for A and B, which leaves the product unchanged).
+// fp64: warp tiles of 32 x 32 in DMMA.8x8x4 fragments (fp64 tensor cores; wgmma has no f64 type), two kernels:
+//   v3  K >= 512 and K % 32 == 0 (the trailing updates): one 128 x 64 tile per CTA, 8 warps, two CTAs per SM,
+//       BK = 32 x 2 stages;
+//   v2  every other K: 128 x 128 tiles, 16 warps, one CTA per SM, persistent over the tiles when K < 512;
+//       BK = 32 x 3 stages when K % 32 == 0, else 16 x 4.
+//   Operands are staged by a cp.async (LDGSTS) ring into a FRAGMENT-MAJOR shared-memory layout: the 16-byte granule
+//   holding (row, k = 2j, 2j+1) is stored where lane (row % 8) * 4 + j of the owning 8-row block reads it, so every
+//   fragment load is one conflict-free, warp-contiguous LDS.128 that feeds TWO DMMAs (the even-k one and the odd-k one --
+//   the k order inside a k-group of 8 is permuted identically for A and B, which leaves the product unchanged).
 //   Roofline: fp64 tensor pipe (measured 37.1 TFLOP/s DMMA peak); algorithmic flops 2 M N K (M N K for lower).
-// fp32: classic register-tiled FFMA kernel (8 x 8 micro-tiles), double-buffered.
-#include <stdlib.h>
-
+//   Large batch-1 products go to the int8-slice emulation (gemm_oz.cu) instead when the caller enabled it.
+// fp32: the 3xTF32 wgmma kernel (gemm_tc32.cu) where its shape rules allow, else a register-tiled FFMA kernel (8 x 8
+//   micro-tiles), double-buffered.
 #include <vector>
 
 #include "common.cuh"
 
 namespace gpk {
 
-constexpr int GM_BM = 128, GM_BN = 128, GM_BK = 16, GM_STAGES = 4, GM_THREADS = 256;
-constexpr int GM_STAGE_ELEMS = GM_BM * GM_BK;  // per operand per stage
+constexpr int GM_BM = 128, GM_BN = 128, GM_BK = 16, GM_THREADS = 256;
 
 template <typename T>
 struct GemmParams {
@@ -47,102 +49,6 @@ __device__ __forceinline__ void tile_coords(int id, int tiles_m, int tiles_n, in
   tn = r / gsize;
 }
 
-__global__ void __launch_bounds__(GM_THREADS, 1) gemm_nt_f64_kernel(const GemmParams<double> p) {
-  int tm, tn;
-  tile_coords(blockIdx.x, p.tiles_m, p.tiles_n, tm, tn);
-  if (p.lower && tn > tm) return;
-  const int b = blockIdx.y;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int wm = warp >> 2, wn = warp & 3;  // 2 x 4 warps; warp tile 64 x 32
-
-  extern __shared__ __align__(16) double gm_smem[];
-  double* As = gm_smem;
-  double* Bs = gm_smem + GM_STAGES * GM_STAGE_ELEMS;
-
-  const double* Ag = p.A + (int64_t)b * p.a_bs + (int64_t)tm * GM_BM * p.lda;
-  const double* Bg = p.B + (int64_t)b * p.b_bs + (int64_t)tn * GM_BN * p.ldb;
-
-  // each thread copies 4 granules of A and 4 of B per stage: rows (tid / 8) + 32 i, granule g = tid % 8
-  const int ld_row = tid >> 3, ld_g = tid & 7;
-  const int ld_slot = ((ld_g >> 2) * 32 + (ld_row & 7) * 4 + (ld_g & 3)) * 2;  // + (row / 8) * 128 per row block
-  auto load_stage = [&](int slot, int kt) {
-    const int64_t koff = (int64_t)kt * GM_BK + ld_g * 2;
-    double* as = As + slot * GM_STAGE_ELEMS;
-    double* bs = Bs + slot * GM_STAGE_ELEMS;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int row = ld_row + 32 * i;
-      const int dst = (row >> 3) * 128 + ld_slot;
-      cp_async16(as + dst, Ag + (int64_t)row * p.lda + koff);
-      cp_async16(bs + dst, Bg + (int64_t)row * p.ldb + koff);
-    }
-  };
-
-  double acc[8][4][2];
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
-
-  const int KT = (int)(p.K / GM_BK);
-#pragma unroll
-  for (int s = 0; s < GM_STAGES - 1; ++s) {
-    if (s < KT) load_stage(s, s);
-    cp_async_commit();
-  }
-
-  for (int kt = 0; kt < KT; ++kt) {
-    cp_async_wait<GM_STAGES - 2>();
-    __syncthreads();
-    {
-      const int nk = kt + GM_STAGES - 1;
-      if (nk < KT) load_stage(nk % GM_STAGES, nk);
-      cp_async_commit();
-    }
-    const double* as = As + (kt % GM_STAGES) * GM_STAGE_ELEMS + (wm * 8) * 128 + lane * 2;
-    const double* bs = Bs + (kt % GM_STAGES) * GM_STAGE_ELEMS + (wn * 4) * 128 + lane * 2;
-#pragma unroll
-    for (int k8 = 0; k8 < 2; ++k8) {
-      double2 a[8], bb[4];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) a[i] = *reinterpret_cast<const double2*>(as + i * 128 + k8 * 64);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) bb[j] = *reinterpret_cast<const double2*>(bs + j * 128 + k8 * 64);
-      // even-k pass over all 32 accumulators, then the odd-k pass: dependent DMMAs are 32 instructions apart
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) dmma884(acc[i][j][0], acc[i][j][1], a[i].x, bb[j].x);
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) dmma884(acc[i][j][0], acc[i][j][1], a[i].y, bb[j].y);
-    }
-  }
-  cp_async_wait<0>();
-
-  // epilogue: lane holds C[row = lane / 4][col = 2 (lane % 4) + {0, 1}] of every 8 x 8 fragment
-  double* Cg = p.C + (int64_t)b * p.c_bs + ((int64_t)tm * GM_BM + wm * 64 + (lane >> 2)) * p.ldc +
-               (int64_t)tn * GM_BN + wn * 32 + 2 * (lane & 3);
-  const double alpha = p.alpha, beta = p.beta;
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      double2* cp = reinterpret_cast<double2*>(Cg + (int64_t)i * 8 * p.ldc + j * 8);
-      double2 v;
-      if (beta != 0.0) {
-        const double2 old = *cp;
-        v.x = fma(alpha, acc[i][j][0], beta * old.x);
-        v.y = fma(alpha, acc[i][j][1], beta * old.y);
-      } else {
-        v.x = alpha * acc[i][j][0];
-        v.y = alpha * acc[i][j][1];
-      }
-      *cp = v;
-    }
-}
-
 // ---- fp64 v2: persistent CTAs, 16 warps, operand prefetch running across tile boundaries ----------------------------
 // One CTA per SM loops over the valid output tiles (static striding over a grouped rasterisation that keeps the A/B
 // panels of concurrently processed tiles in L2).  The cp.async pipeline treats the CTA's whole sequence of
@@ -151,7 +57,6 @@ __global__ void __launch_bounds__(GM_THREADS, 1) gemm_nt_f64_kernel(const GemmPa
 // 16 warps (4 x 4, warp tile 32 x 32) put four warps on every SM sub-partition: enough independent DMMA chains to keep
 // the fp64 tensor pipe busy across the per-k-tile barrier and the LDS latency (the 8-warp version idles it ~17 %).
 constexpr int G2_THREADS = 512;
-constexpr int G2_MAX_GROUPS = 448;
 
 struct Gemm2Params {
   int64_t K;
@@ -164,8 +69,13 @@ struct Gemm2Params {
   int64_t ldc, c_bs;
   int32_t lower, tiles_m, tiles_n, n_groups;
   int32_t tiles_per_batch, total_tiles;
-  int32_t group_prefix[G2_MAX_GROUPS + 1];  // lower mode: first valid-tile index of every 8-row group
 };
+
+// lower mode: the valid tiles of tile rows 0 .. rows - 1 (row i holds min(i + 1, tiles_n) of them)
+__host__ __device__ __forceinline__ int g2_lower_tiles(int rows, int tiles_n) {
+  const int tri = rows < tiles_n ? rows : tiles_n;
+  return tri * (tri + 1) / 2 + (rows - tri) * tiles_n;
+}
 
 __device__ __forceinline__ void g2_decode(const Gemm2Params& p, int idx, int& b, int& tm, int& tn) {
   b = idx / p.tiles_per_batch;
@@ -174,9 +84,9 @@ __device__ __forceinline__ void g2_decode(const Gemm2Params& p, int idx, int& b,
     tile_coords(r, p.tiles_m, p.tiles_n, tm, tn);
     return;
   }
-  int g = 0;
-  while (g + 1 < p.n_groups && p.group_prefix[g + 1] <= r) ++g;
-  r -= p.group_prefix[g];
+  int g = 0;  // the 8-row group of tile r
+  while (g + 1 < p.n_groups && g2_lower_tiles(8 * (g + 1), p.tiles_n) <= r) ++g;
+  r -= g2_lower_tiles(8 * g, p.tiles_n);
   const int first = g * 8;
   const int gsize = min(p.tiles_m - first, 8);
   const int c0 = min(first, p.tiles_n);  // columns left of the group's diagonal block: all gsize rows valid
@@ -584,104 +494,47 @@ int gemm_nt_f64(int64_t M, int64_t N, int64_t K, double alpha, const double* A, 
     if (rc == 1) return 0;
   }
   const int32_t tiles_m = (int32_t)(M / GM_BM), tiles_n = (int32_t)(N / GM_BN);
-  const int smem = 2 * GM_STAGES * GM_STAGE_ELEMS * (int)sizeof(double);
-  const int n_groups = (tiles_m + 7) / 8;
-  static const bool force_v1 = getenv("GPK_GEMM_V1") != nullptr;
-  static const int v3_mode = getenv("GPK_GEMM_V3") ? atoi(getenv("GPK_GEMM_V3")) : 1;  // 0 off, 1 BK32x2, 2 BK16x4
-  if (!force_v1 && v3_mode && K >= 512 && K % 32 == 0) {
+  if (K >= 512 && K % 32 == 0) {
     GemmParams<double> p3{M, N, K, alpha, beta, A, lda, a_bs, B, ldb, b_bs, C, ldc, c_bs, lower, tiles_m,
                           (int32_t)(N / G3_BN)};
-    constexpr int smem_a = (GM_BM + G3_BN) * 32 * 2 * (int)sizeof(double);  // BK = 32, 2 stages: 96 KB
-    constexpr int smem_b = (GM_BM + G3_BN) * 16 * 4 * (int)sizeof(double);  // BK = 16, 4 stages: 96 KB
-    static bool attr3_set = false;
-    if (!attr3_set) {
-      cudaError_t e = cudaFuncSetAttribute(gemm_nt_f64_v3_kernel<32, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_a);
-      if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(gemm_nt_f64_v3_kernel<16, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_b);
-      if (e != cudaSuccess) return -1000 - (int)e;
-      attr3_set = true;
-    }
+    constexpr int smem = (GM_BM + G3_BN) * 32 * 2 * (int)sizeof(double);  // BK = 32, 2 stages: 96 KB
+    if ((rc = opt_in_smem<gemm_nt_f64_v3_kernel<32, 2>>(smem))) return rc;
     dim3 grid3((unsigned)(p3.tiles_m * p3.tiles_n), (unsigned)batch);
     if (g_prof.enabled) {
       const double tn = (double)tiles_n, tmm = (double)tiles_m;
       const double tiles = lower ? (tn * (tn + 1) / 2 + (tmm - tn) * tn) : tmm * tn;  // in 128 x 128 units
       prof_begin(stream, tiles * 2.0 * GM_BM * GM_BN * (double)K * batch);
     }
-    if (v3_mode == 2)
-      gemm_nt_f64_v3_kernel<16, 4><<<grid3, G3_THREADS, smem_b, stream>>>(p3);
-    else
-      gemm_nt_f64_v3_kernel<32, 2><<<grid3, G3_THREADS, smem_a, stream>>>(p3);
+    gemm_nt_f64_v3_kernel<32, 2><<<grid3, G3_THREADS, smem, stream>>>(p3);
     if (g_prof.enabled) prof_end(stream);
     GPK_COUNT_LAUNCH();
     GPK_CHECK_LAUNCH();
     return 0;
   }
-  if (!force_v1 && K > 0 && (!lower || n_groups <= G2_MAX_GROUPS) && (int64_t)tiles_m * tiles_n * batch < (1ll << 30)) {
-    static Gemm2Params q;  // large (group table): filled in place, passed by value at launch
-    q.K = K; q.alpha = alpha; q.beta = beta; q.A = A; q.lda = lda; q.a_bs = a_bs; q.B = B; q.ldb = ldb; q.b_bs = b_bs;
-    q.C = C; q.ldc = ldc; q.c_bs = c_bs; q.lower = lower; q.tiles_m = tiles_m; q.tiles_n = tiles_n;
-    q.n_groups = n_groups;
-    int per_batch;
-    if (lower) {
-      int acc = 0;
-      for (int g = 0; g < n_groups; ++g) {
-        q.group_prefix[g] = acc;
-        const int first = g * 8, gsize = (tiles_m - first < 8) ? tiles_m - first : 8;
-        for (int r = 0; r < gsize; ++r) acc += (first + r + 1 < tiles_n) ? first + r + 1 : tiles_n;
-      }
-      q.group_prefix[n_groups] = acc;
-      per_batch = acc;
-    } else {
-      per_batch = tiles_m * tiles_n;
-    }
-    q.tiles_per_batch = per_batch;
-    q.total_tiles = per_batch * batch;
-    static int num_sms = 0;
-    static bool attr2_set = false;
-    constexpr int smem16 = 2 * 4 * GM_BM * 16 * (int)sizeof(double);  // BK = 16, 4 stages: 128 KB
-    constexpr int smem32 = 2 * 3 * GM_BM * 32 * (int)sizeof(double);  // BK = 32, 3 stages: 192 KB
-    if (!attr2_set) {
-      int dev = 0;
-      cudaGetDevice(&dev);
-      cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-      cudaError_t e = cudaFuncSetAttribute(gemm_nt_f64_v2_kernel<16, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           smem16);
-      if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(gemm_nt_f64_v2_kernel<32, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem32);
-      if (e != cudaSuccess) return -1000 - (int)e;
-      attr2_set = true;
-    }
-    // Small-K updates (panel steps) run persistent: the cross-tile prefetch hides their per-tile prologue.  Large-K
-    // trailing updates launch one CTA per tile instead, so that CTAs retire continuously and the high-priority
-    // look-ahead kernels of the side stream can get SMs while the update is in flight.
-    static const bool force_persistent = getenv("GPK_GEMM_PERSISTENT") != nullptr;
-    static const bool force_bk16 = getenv("GPK_GEMM_BK16") != nullptr;
-    const bool persistent = force_persistent || K < 512;
-    const int grid = (persistent && q.total_tiles > num_sms) ? num_sms : q.total_tiles;
-    // (the in-situ profile covers the dominant kernel only -- the v3 trailing-update GEMM)
-    if (K % 32 == 0 && !force_bk16)
-      gemm_nt_f64_v2_kernel<32, 3><<<grid, G2_THREADS, smem32, stream>>>(q);
-    else
-      gemm_nt_f64_v2_kernel<16, 4><<<grid, G2_THREADS, smem16, stream>>>(q);
-    GPK_COUNT_LAUNCH();
-    GPK_CHECK_LAUNCH();
-    return 0;
+  if ((M / GM_BM) * (N / GM_BN) * batch >= (1ll << 30)) return GPK_ERR_UNSUPPORTED;  // v2 counts tiles in int32
+  Gemm2Params q{K, alpha, beta, A, lda, a_bs, B, ldb, b_bs, C, ldc, c_bs, lower, tiles_m, tiles_n, (tiles_m + 7) / 8};
+  q.tiles_per_batch = lower ? g2_lower_tiles(tiles_m, tiles_n) : tiles_m * tiles_n;
+  q.total_tiles = q.tiles_per_batch * batch;
+  static const int num_sms = [] {
+    int dev = 0, n = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    return n;
+  }();
+  constexpr int smem16 = 2 * 4 * GM_BM * 16 * (int)sizeof(double);  // BK = 16, 4 stages: 128 KB
+  constexpr int smem32 = 2 * 3 * GM_BM * 32 * (int)sizeof(double);  // BK = 32, 3 stages: 192 KB
+  // Small-K updates (panel steps) run persistent: the cross-tile prefetch hides their per-tile prologue.  Large-K
+  // updates launch one CTA per tile instead, so that CTAs retire continuously and the high-priority look-ahead kernels
+  // of the side stream can get SMs while the update is in flight.
+  const int grid = (K < 512 && q.total_tiles > num_sms) ? num_sms : q.total_tiles;
+  // (the in-situ profile covers the dominant kernel only -- the v3 trailing-update GEMM)
+  if (K % 32 == 0) {
+    if ((rc = opt_in_smem<gemm_nt_f64_v2_kernel<32, 3>>(smem32))) return rc;
+    gemm_nt_f64_v2_kernel<32, 3><<<grid, G2_THREADS, smem32, stream>>>(q);
+  } else {
+    if ((rc = opt_in_smem<gemm_nt_f64_v2_kernel<16, 4>>(smem16))) return rc;
+    gemm_nt_f64_v2_kernel<16, 4><<<grid, G2_THREADS, smem16, stream>>>(q);
   }
-  GemmParams<double> p{M, N, K, alpha, beta, A, lda, a_bs, B, ldb, b_bs, C, ldc, c_bs, lower, tiles_m, tiles_n};
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_nt_f64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return -1000 - (int)e;
-    attr_set = true;
-  }
-  dim3 grid((unsigned)(p.tiles_m * p.tiles_n), (unsigned)batch);
-  if (g_prof.enabled) {
-    const double tn = (double)p.tiles_n, tmm = (double)p.tiles_m;
-    const double tiles = lower ? (tn * (tn + 1) / 2 + (tmm - tn) * tn) : tmm * tn;  // lower: tile_m >= tile_n
-    prof_begin(stream, tiles * 2.0 * GM_BM * GM_BN * (double)K * batch);
-  }
-  gemm_nt_f64_kernel<<<grid, GM_THREADS, smem, stream>>>(p);
-  if (g_prof.enabled) prof_end(stream);
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();
   return 0;

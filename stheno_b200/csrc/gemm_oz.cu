@@ -30,7 +30,6 @@
 // every tile of the trailing update.  Every inexact step is ONE correctly rounded fp64 operation, so the result equals a
 // NumPy integer model of the algorithm bit for bit (tests/_oz_model.py, tests/test_emulation.py).
 #include <cuda.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -393,13 +392,7 @@ int oz_launch_gemm(int64_t M, int64_t N, int64_t K, double alpha, const int8_t* 
   CUtensorMap mA, mB;
   if (!oz_make_map(&mA, planesA, K, capA, strideA, S, OZ_BM) || !oz_make_map(&mB, planesB, K, capB, strideB, S, OZ_HN))
     return GPK_ERR_UNSUPPORTED;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e =
-        cudaFuncSetAttribute(oz_gemm_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, OzCfg<S>::SMEM_BYTES);
-    if (e != cudaSuccess) return -1000 - (int)e;
-    attr_set = true;
-  }
+  if (const int rc = opt_in_smem<oz_gemm_kernel<S>>(OzCfg<S>::SMEM_BYTES)) return rc;
   if (beta != 0.0 && beta != 1.0) {  // the kernel adds into C (or overwrites it): apply any other beta first
     if (M > 65535) return GPK_ERR_UNSUPPORTED;
     oz_scale_kernel<<<dim3((unsigned)((N + 255) / 256), (unsigned)M), 256, 0, stream>>>(C, ldc, M, N, beta);
@@ -408,16 +401,15 @@ int oz_launch_gemm(int64_t M, int64_t N, int64_t K, double alpha, const int8_t* 
   const int32_t tiles_m = (int32_t)(M / OZ_BM), tiles_n = (int32_t)(N / OZ_BN);
   const int32_t tri_rows = lower ? (tiles_m < tiles_n / 2 ? tiles_m : tiles_n / 2) : 0;
   const int32_t total = lower ? tri_rows * (tri_rows + 1) + (tiles_m - tri_rows) * tiles_n : tiles_m * tiles_n;
-  static const int force_tpc = getenv("GPK_OZ_TPC") ? atoi(getenv("GPK_OZ_TPC")) : 0;
-  int32_t tpc = force_tpc > 0 ? force_tpc : total / 264;  // >= 2 waves of CTAs over the H100's 132 SMs before CTAs grow
-  static const int env_cap = getenv("GPK_OZ_TPC_CAP") ? atoi(getenv("GPK_OZ_TPC_CAP")) : 0;  // experiments
-  static const int env_band = getenv("GPK_OZ_BAND") ? atoi(getenv("GPK_OZ_BAND")) : 0;
+  // tiles per CTA: >= 2 waves of CTAs over the H100's 132 SMs before CTAs grow, and CTAs stay short-lived (look-ahead
+  // streams need SMs every few tens of us)
+  const int32_t tpc_cap = K > 512 ? 2 : 4;
+  int32_t tpc = total / 264;
+  tpc = tpc < 1 ? 1 : (tpc > tpc_cap ? tpc_cap : tpc);
   // band height of the tile order: as many tile rows as keep the band's A slices (128 K S bytes per tile row) within ~12 MB
   // of the H100's 50 MB L2, at most 16 (K = 1024, S = 7: 13 rows = 11.4 MB; the K = 8192 products of the triangular solves: 1-2 rows)
   int32_t band = (int32_t)((12ll << 20) / (128ll * K * S));
-  band = env_band > 0 ? env_band : (band < 1 ? 1 : (band > 16 ? 16 : band));
-  const int32_t tpc_cap = env_cap > 0 ? env_cap : (K > 512 ? 2 : 4);  // CTAs stay short-lived (look-ahead streams need SMs every few tens of us)
-  tpc = tpc < 1 ? 1 : (tpc > tpc_cap && force_tpc <= 0 ? tpc_cap : tpc);
+  band = band < 1 ? 1 : (band > 16 ? 16 : band);
   OzParams p{alpha, C, scA + rowA, scB + rowB, ldc, (int32_t)rowA, (int32_t)rowB, (int32_t)(K / OZ_BK), lower,
              tiles_m, tiles_n, total, tpc, tri_rows, beta != 0.0 ? 1 : 0, band};
   // profile: algorithmic (fp64-equivalent) flops of the tiles computed; the int8 work is S (S + 1) / 2 times that

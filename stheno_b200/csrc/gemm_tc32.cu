@@ -14,7 +14,6 @@
 // Used by the fp32 (batched) Cholesky for its trailing / panel updates (BASELINE config 3).  The fp64 default path
 // cannot use this unit (no f64 wgmma); see DESIGN.md section 8.
 #include <cuda.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -213,12 +212,7 @@ static int launch_tc(int64_t M, int64_t N, int64_t K, float alpha, const float* 
                      int32_t batch, cudaStream_t stream) {
   CUtensorMap mA, mB;
   if (!make_map(&mA, A, K, M, lda, a_bs, batch, TC_BM) || !make_map(&mB, B, K, N, ldb, b_bs, batch, TC_BN)) return 0;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_nt_f32_tc_kernel<CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES);
-    if (e != cudaSuccess) return -1000 - (int)e;
-    attr_set = true;
-  }
+  if (const int rc = opt_in_smem<gemm_nt_f32_tc_kernel<CT>>(TC_SMEM_BYTES)) return rc;
   TcParams p{alpha, beta, C, ldc, c_bs, (int32_t)K, lower, (int32_t)(M / TC_BM), (int32_t)(N / TC_BN)};
   dim3 grid((unsigned)(p.tiles_m * p.tiles_n), (unsigned)batch);
   gemm_nt_f32_tc_kernel<CT><<<grid, TC_GEMM_THREADS, TC_SMEM_BYTES, stream>>>(mA, mB, p);
@@ -232,8 +226,7 @@ static int launch_tc(int64_t M, int64_t N, int64_t K, float alpha, const float* 
 int gemm_nt_f32_tc(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t lda, int64_t a_bs, const float* B,
                    int64_t ldb, int64_t b_bs, float beta, float* C, int64_t ldc, int64_t c_bs, int32_t lower,
                    int32_t batch, cudaStream_t stream) {
-  static const bool disabled = getenv("GPK_F32_FFMA") != nullptr;
-  if (disabled || K < 128 || K % TC_BK || M % TC_BM || N % TC_BN) return 0;
+  if (K < 128 || K % TC_BK || M % TC_BM || N % TC_BN) return 0;
   if (lda % 4 || ldb % 4 || ldc % 4 || (batch > 1 && (a_bs % 4 || b_bs % 4))) return 0;
   if ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B) | reinterpret_cast<uintptr_t>(C)) % 16) return 0;
   return launch_tc<float>(M, N, K, alpha, A, lda, a_bs, B, ldb, b_bs, beta, C, ldc, c_bs, lower, batch, stream);

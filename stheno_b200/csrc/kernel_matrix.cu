@@ -12,8 +12,6 @@
 // Reference arithmetic replaced: mlkernels.pairwise for EQ/Matern/Linear/Delta and Scaled/Sum/Product/Stretched
 // (call sites stheno/model/fdd.py:79, stheno/model/observations.py:139,285,286), Dense + Diagonal (fdd.py:79)
 // and B.reg's "+ epsilon I" (README.md:820-830).
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace gpk {
@@ -342,114 +340,13 @@ __device__ __forceinline__ float fast_factor<float, GPK_MATERN52>(float d2, int 
   return (1.0f + s + 1.6666666666666667f * d2) * expf(-s);
 }
 
-// ---- one tile per CTA (round-2 first version; GPK_K1_ONE_TILE=1 selects it for A/B comparisons) ----
-template <typename T, int KIND>
-__global__ void __launch_bounds__(KM_THREADS, 2) kernel_matrix_fast1_kernel(const KmParams p) {
-  const int tile_c = blockIdx.x, tile_r = blockIdx.y, b = blockIdx.z;
-  const bool lower = p.flags & GPK_KM_LOWER;
-  if (lower && (tile_c >> 1) > (tile_r >> 1)) return;
-  const bool same_obj = p.flags & GPK_KM_SAME;
-  const int d = p.d;
-  const int g = p.desc.fac_group[0];
-  const int64_t r0 = (int64_t)tile_r * KM_TILE, c0 = (int64_t)tile_c * KM_TILE;
-
-  extern __shared__ __align__(16) unsigned char km_smem[];
-  __shared__ __align__(8) uint64_t bar;
-  __shared__ double tab[64];
-  T* xs = reinterpret_cast<T*>(km_smem);  // [64][d]
-  T* ys = xs + (size_t)KM_TILE * d;       // [64][d]
-  T* yt = ys + (size_t)KM_TILE * d;       // [d][65]
-  const T* xg = static_cast<const T*>(p.xg) + (int64_t)b * p.x_bstride + g * p.xg_gstride + r0 * d;
-  const T* yg = static_cast<const T*>(p.yg) + (int64_t)b * p.y_bstride + g * p.yg_gstride + c0 * d;
-  if (sizeof(T) == 8 && threadIdx.x < 64) tab[threadIdx.x] = exp2((double)threadIdx.x * 0.015625);
-
-  const int xr = (int)max((int64_t)0, min((int64_t)KM_TILE, p.n - r0));
-  const int yr = (int)max((int64_t)0, min((int64_t)KM_TILE, p.n2 - c0));
-  const uint32_t xbytes = (uint32_t)xr * d * sizeof(T), ybytes = (uint32_t)yr * d * sizeof(T);
-  const bool bulk = (xbytes % 16 == 0) && (ybytes % 16 == 0) && ((KM_TILE * d * sizeof(T)) % 16 == 0) &&
-                    (reinterpret_cast<uintptr_t>(xg) % 16 == 0) && (reinterpret_cast<uintptr_t>(yg) % 16 == 0);
-  if (bulk) {
-    if (threadIdx.x == 0) {
-      mbar_init(&bar, 1);
-      fence_mbar_init();
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      mbar_arrive_expect_tx(&bar, xbytes + ybytes);
-      if (xbytes) bulk_copy_g2s(xs, xg, xbytes, &bar);
-      if (ybytes) bulk_copy_g2s(ys, yg, ybytes, &bar);
-    }
-    mbar_wait(&bar, 0);
-  } else {
-    for (int i = threadIdx.x; i < xr * d; i += KM_THREADS) xs[i] = xg[i];
-    for (int i = threadIdx.x; i < yr * d; i += KM_THREADS) ys[i] = yg[i];
-    __syncthreads();
-  }
-  for (int idx = threadIdx.x; idx < yr * d; idx += KM_THREADS) {
-    const int c = idx / d, k = idx - c * d;
-    yt[(size_t)k * (KM_TILE + 1) + c] = ys[idx];
-  }
-  __syncthreads();
-
-  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  T d2[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) d2[i][j] = T(0);
-  const T* xr_ = xs + (size_t)(ty * 4) * d;
-  const T* yc_ = yt + tx;
-#pragma unroll 2
-  for (int k = 0; k < d; ++k) {
-    T xv[4], yv[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) xv[i] = xr_[i * d + k];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) yv[j] = yc_[(size_t)k * (KM_TILE + 1) + 16 * j];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const T df = xv[i] - yv[j];
-        d2[i][j] = fma(df, df, d2[i][j]);
-      }
-  }
-
-  T* out = static_cast<T*>(p.out) + (int64_t)b * p.o_bstride;
-  const T* nv = p.noise_vec ? static_cast<const T*>(p.noise_vec) + (int64_t)b * p.nv_bstride : nullptr;
-  const bool pad_id = p.flags & GPK_KM_PAD_IDENTITY;
-  const T coef = (T)p.desc.coef[0];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int64_t r = r0 + ty * 4 + i;
-    if (r >= p.rows_out) continue;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int64_t c = c0 + tx + 16 * j;
-      if (c >= p.cols_out) continue;
-      T val;
-      if (r >= p.n || c >= p.n2) {
-        val = (pad_id && r == c) ? T(1) : T(0);
-      } else {
-        val = coef * fast_factor<T, KIND>(d2[i][j], d, tab);
-        if (same_obj && r == c) {
-          val += (T)p.noise_scalar;
-          if (nv) val += nv[r];
-          val += (T)p.jitter;
-        }
-      }
-      out[r * p.ldo + c] = val;
-    }
-  }
-}
-
 constexpr int KM_STRIP = 8;  // column tiles per CTA of the fast kernel
 
 // One CTA = one row tile x a strip of up to KM_STRIP column tiles.  The x rows are staged once; the y rows of tile c + 1 are
 // fetched by the TMA engine (double-buffered, one mbarrier per buffer) while tile c is evaluated, so the bulk-copy latency,
 // the transposition and the barriers of a tile hide under the arithmetic of its predecessor (round-2 ncu of the
 // one-tile-per-CTA version: FP64 pipe 35 % busy with 3 CTAs per SM -- the per-tile prologue was as long as the tile's math).
-// n = 16384, lower: 0.499 ms against 0.585 ms for the one-tile kernel (1.22 ms for the generic descriptor kernel).
+// n = 16384, lower: 0.499 ms against 0.585 ms for one tile per CTA (1.22 ms for the generic descriptor kernel).
 template <typename T, int KIND>
 __global__ void __launch_bounds__(KM_THREADS, 3) kernel_matrix_fast_kernel(const KmParams p) {
   const int tile_r = blockIdx.y, b = blockIdx.z;
@@ -586,6 +483,15 @@ __global__ void __launch_bounds__(KM_THREADS, 3) kernel_matrix_fast_kernel(const
   }
 }
 
+template <typename T, int KIND>
+static int launch_fast(const KmParams& p, dim3 grid, int smem, void* stream) {
+  if (const int rc = opt_in_smem<kernel_matrix_fast_kernel<T, KIND>>(smem)) return rc;
+  kernel_matrix_fast_kernel<T, KIND><<<grid, KM_THREADS, smem, (cudaStream_t)stream>>>(p);
+  GPK_COUNT_LAUNCH();
+  GPK_CHECK_LAUNCH();
+  return 0;
+}
+
 template <typename T>
 static int launch_kernel_matrix(const gpk_kernel_desc* desc, const T* xg, int64_t xg_gstride, int64_t x_bstride,
                                 int64_t n, const T* yg, int64_t yg_gstride, int64_t y_bstride, int64_t n2, int32_t d,
@@ -622,40 +528,26 @@ static int launch_kernel_matrix(const gpk_kernel_desc* desc, const T* xg, int64_
   dim3 grid((unsigned)((p.cols_out + KM_TILE - 1) / KM_TILE), (unsigned)((p.rows_out + KM_TILE - 1) / KM_TILE),
             (unsigned)batch);
   if (grid.y > 65535 || grid.z > 65535) return GPK_ERR_UNSUPPORTED;
-  // one stationary factor: the specialised kernel (GPK_K1_GENERIC=1 forces the generic one, for A/B comparisons)
-  static const bool force_generic = getenv("GPK_K1_GENERIC") != nullptr;
+  // one stationary factor: the specialised kernel
   const int kind0 = desc->fac_kind[0];
-  if (!force_generic && desc->n_terms == 1 && desc->term_begin[1] - desc->term_begin[0] == 1 && kind0 >= GPK_EQ &&
-      kind0 <= GPK_MATERN52 && desc->fac_group[0] >= 0 && desc->fac_group[0] < desc->n_groups) {
-    static const bool one_tile = getenv("GPK_K1_ONE_TILE") != nullptr;
-    const size_t fsmem = ((size_t)(one_tile ? 2 : 3) * KM_TILE * d + (size_t)d * (KM_TILE + 1)) * sizeof(T);
+  if (desc->n_terms == 1 && desc->term_begin[1] - desc->term_begin[0] == 1 && kind0 >= GPK_EQ && kind0 <= GPK_MATERN52 &&
+      desc->fac_group[0] >= 0 && desc->fac_group[0] < desc->n_groups) {
+    // x rows, two y buffers and the transposed y tile
+    const size_t fsmem = ((size_t)3 * KM_TILE * d + (size_t)d * (KM_TILE + 1)) * sizeof(T);
     if (fsmem <= 96 * 1024) {
-      void (*fk)(const KmParams) = nullptr;
+      const dim3 fgrid((grid.x + KM_STRIP - 1) / KM_STRIP, grid.y, grid.z);
       switch (kind0) {
-        case GPK_EQ: fk = one_tile ? kernel_matrix_fast1_kernel<T, GPK_EQ> : kernel_matrix_fast_kernel<T, GPK_EQ>; break;
-        case GPK_MATERN12: fk = one_tile ? kernel_matrix_fast1_kernel<T, GPK_MATERN12> : kernel_matrix_fast_kernel<T, GPK_MATERN12>; break;
-        case GPK_MATERN32: fk = one_tile ? kernel_matrix_fast1_kernel<T, GPK_MATERN32> : kernel_matrix_fast_kernel<T, GPK_MATERN32>; break;
-        default: fk = one_tile ? kernel_matrix_fast1_kernel<T, GPK_MATERN52> : kernel_matrix_fast_kernel<T, GPK_MATERN52>; break;
+        case GPK_EQ: return launch_fast<T, GPK_EQ>(p, fgrid, (int)fsmem, stream);
+        case GPK_MATERN12: return launch_fast<T, GPK_MATERN12>(p, fgrid, (int)fsmem, stream);
+        case GPK_MATERN32: return launch_fast<T, GPK_MATERN32>(p, fgrid, (int)fsmem, stream);
+        default: return launch_fast<T, GPK_MATERN52>(p, fgrid, (int)fsmem, stream);
       }
-      if (fsmem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(fk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem);
-        if (e != cudaSuccess) return -1000 - (int)e;
-      }
-      dim3 fgrid(one_tile ? grid.x : (grid.x + KM_STRIP - 1) / KM_STRIP, grid.y, grid.z);
-      fk<<<fgrid, KM_THREADS, fsmem, (cudaStream_t)stream>>>(p);
-      GPK_COUNT_LAUNCH();
-      GPK_CHECK_LAUNCH();
-      return 0;
     }
   }
   const size_t smem = ((size_t)2 * desc->n_groups * KM_TILE * d + (size_t)desc->n_groups * d * (KM_TILE + 1)) * sizeof(T);
   if (smem > 200 * 1024) return GPK_ERR_UNSUPPORTED;
-  auto kern = kernel_matrix_kernel<T>;
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return -1000 - (int)e;
-  }
-  kern<<<grid, KM_THREADS, smem, (cudaStream_t)stream>>>(p);
+  if (const int rc = opt_in_smem<kernel_matrix_kernel<T>>((int)smem)) return rc;
+  kernel_matrix_kernel<T><<<grid, KM_THREADS, smem, (cudaStream_t)stream>>>(p);
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();
   return 0;

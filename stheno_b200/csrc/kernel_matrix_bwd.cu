@@ -266,13 +266,9 @@ static int launch_kernel_matrix_bwd(const gpk_kernel_desc* desc, const T* xg, in
   const int dc = fit < (size_t)d ? (int)fit : d;
   const int chunks = (d + dc - 1) / dc;
   const size_t smem = rows_bytes + (size_t)dc * dim_bytes;
-  auto kern = kernel_matrix_bwd_kernel<T>;
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return -1000 - (int)e;
-  }
+  if (const int rc = opt_in_smem<kernel_matrix_bwd_kernel<T>>((int)smem)) return rc;
   dim3 grid((unsigned)((n + KB_TILE - 1) / KB_TILE), (unsigned)batch, (unsigned)chunks);
-  kern<<<grid, KB_THREADS, smem, (cudaStream_t)stream>>>(p, dc);
+  kernel_matrix_bwd_kernel<T><<<grid, KB_THREADS, smem, (cudaStream_t)stream>>>(p, dc);
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();
   return 0;

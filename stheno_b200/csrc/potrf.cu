@@ -1,6 +1,6 @@
 // K2 / K3: blocked right-looking Cholesky (lower, row-major, in place) and the recursive triangular solve.
 //
-//   potrf      two-level blocking: 128-wide leaf steps inside 512-wide outer panels (GPK_NB_OUTER).  Per leaf step
+//   potrf      two-level blocking: 128-wide leaf steps inside 512-wide outer panels (NB_OUTER).  Per leaf step
 //                (1) potrf_leaf  : one CTA factorises the 128 x 128 diagonal block (log-det and info folded in): fp64 = the
 //                                  recursive shared-memory kernel (4 x 4 sub-blocks of 32 x 32, single-warp in-register
 //                                  factorisation of each diagonal sub-block, 33 us); fp32 = the register-tiled kernel
@@ -427,6 +427,7 @@ trsm_leaf_kernel(const T* __restrict__ L, int64_t ldl, int64_t l_bs, T* __restri
 // the next product straight from registers.  256 DMMA + 128 LDS.128 per warp; no shared-memory traffic for A at all.
 constexpr int TC_ROWS = 128;
 constexpr int TC_THREADS = 512;
+constexpr int TC_SMEM = (NB * NB + 8 * 16 * 17) * (int)sizeof(double);  // L11 fragment-major + the diagonal blocks
 
 __device__ __forceinline__ int frag_index(int n, int k) {
   // element (row n, col k) of a 128 x 128 operand in fragment-major layout (16 k8-groups per 8-row block)
@@ -435,14 +436,10 @@ __device__ __forceinline__ int frag_index(int n, int k) {
 
 // T = storage type (double or float).  The arithmetic is always fp64 on the DMMA pipe: for fp32 problems the leaf TRSM is
 // < 2 % of the flops, and doing it in fp64 costs nothing while removing one source of fp32 round-off.
-// With D != nullptr (one CTA per matrix: the 128 rows right below L11) the kernel goes on to the rank-128 update of the
-// next diagonal block, D -= X X^T (lower 8 x 8 blocks), without leaving the SM: the solved rows are still in registers as
-// A-operand fragments and are parked in shared memory (over L11, fragment-major) as the B operand.  That is the whole
-// dependency of the next leaf factorisation in ONE launch (leaf -> this kernel -> next leaf).
 template <typename T>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 trsm_leaf_tc_kernel(const T* __restrict__ L, int64_t ldl, int64_t l_bs, T* __restrict__ B, int64_t ldb, int64_t b_bs,
-                    T* __restrict__ D, int64_t ldd, int64_t d_bs, int32_t rows_per_cta) {
+                    int32_t rows_per_cta) {
   extern __shared__ __align__(16) unsigned char tc_smem[];
   double* Ls = reinterpret_cast<double*>(tc_smem);  // 128 x 128 fragment-major
   double* Ld = Ls + NB * NB;                         // [8][16][17] diagonal blocks (natural layout)
@@ -543,50 +540,15 @@ trsm_leaf_tc_kernel(const T* __restrict__ L, int64_t ldl, int64_t l_bs, T* __res
     Bw[cb * 8] = (T)acc[cb][0];
     Bw[cb * 8 + 1] = (T)acc[cb][1];
   }
-  if (D == nullptr) return;
-
-  // ---- fused rank-128 update of the next diagonal block: D[8w .. 8w+7, 8cb .. 8cb+7] -= X_w X_cb^T for cb <= w ----
-  __syncthreads();  // every warp is done reading L11 from shared memory
-#pragma unroll
-  for (int cb = 0; cb < 16; ++cb)  // fragment (row block = warp, k8 group = cb): lane's double2 at ((w*16+cb)*32+lane)*2
-    *reinterpret_cast<double2*>(Ls + ((warp * 16 + cb) * 32 + lane) * 2) = make_double2(acc[cb][0], acc[cb][1]);
-  __syncthreads();
-  D += (int64_t)blockIdx.y * d_bs;
-  T* Dw = D + (int64_t)(warp * 8 + (lane >> 2)) * ldd + 2 * (lane & 3);
-  // warp w owns w + 1 output blocks: pair the work as (w, 15 - w) would need a second pass; instead split every block's
-  // k range in halves across the two DMMA chains below (independent accumulators), which keeps the pipe full
-#pragma unroll 1
-  for (int cb = 0; cb <= warp; ++cb) {
-    double d0[2] = {0.0, 0.0}, d1[2] = {0.0, 0.0};
-    const double c0 = (double)Dw[cb * 8], c1 = (double)Dw[cb * 8 + 1];
-    const double* Xb = Lf + (cb * 16) * 64;
-#pragma unroll
-    for (int kg = 0; kg < 8; ++kg) {
-      const double2 b0 = *reinterpret_cast<const double2*>(Xb + kg * 64);
-      const double2 b1 = *reinterpret_cast<const double2*>(Xb + (kg + 8) * 64);
-      dmma884(d0[0], d0[1], acc[kg][0], b0.x);
-      dmma884(d1[0], d1[1], acc[kg + 8][0], b1.x);
-      dmma884(d0[0], d0[1], acc[kg][1], b0.y);
-      dmma884(d1[0], d1[1], acc[kg + 8][1], b1.y);
-    }
-    Dw[cb * 8] = (T)(c0 - (d0[0] + d1[0]));
-    Dw[cb * 8 + 1] = (T)(c1 - (d0[1] + d1[1]));
-  }
 }
 
 template <typename T>
 static int launch_trsm_leaf_tc(const T* L, int64_t ldl, int64_t l_bs, T* B, int64_t ldb, int64_t b_bs, int64_t rows,
                                int32_t batch, cudaStream_t stream) {
   if (rows == 0) return 0;
-  const int smem = (NB * NB + 8 * 16 * 17) * (int)sizeof(double);
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(trsm_leaf_tc_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return -1000 - (int)e;
-    attr_set = true;
-  }
+  if (const int rc = opt_in_smem<trsm_leaf_tc_kernel<T>>(TC_SMEM)) return rc;
   dim3 grid((unsigned)(rows / TC_ROWS), (unsigned)batch);
-  trsm_leaf_tc_kernel<T><<<grid, TC_THREADS, smem, stream>>>(L, ldl, l_bs, B, ldb, b_bs, nullptr, 0, 0, TC_ROWS);
+  trsm_leaf_tc_kernel<T><<<grid, TC_THREADS, TC_SMEM, stream>>>(L, ldl, l_bs, B, ldb, b_bs, TC_ROWS);
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();
   return 0;
@@ -635,23 +597,8 @@ diag_syrk_kernel(const T* __restrict__ X, int64_t ldx, int64_t x_bs, T* __restri
 template <typename T>
 static int launch_diag_step(const T* L, int64_t ldl, int64_t l_bs, T* B, int64_t ldb, int64_t b_bs, T* D, int64_t ldd,
                             int64_t d_bs, int32_t batch, cudaStream_t stream) {
-  const int smem = (NB * NB + 8 * 16 * 17) * (int)sizeof(double);
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(trsm_leaf_tc_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return -1000 - (int)e;
-    attr_set = true;
-  }
-  static const bool fused = getenv("GPK_DIAG_FUSED") != nullptr;  // one-CTA variant (solve + update in one launch)
-  if (fused) {
-    trsm_leaf_tc_kernel<T><<<dim3(1, (unsigned)batch), TC_THREADS, smem, stream>>>(L, ldl, l_bs, B, ldb, b_bs, D, ldd, d_bs,
-                                                                                  TC_ROWS);
-    GPK_COUNT_LAUNCH();
-    GPK_CHECK_LAUNCH();
-    return 0;
-  }
-  trsm_leaf_tc_kernel<T><<<dim3(4, (unsigned)batch), TC_THREADS, smem, stream>>>(L, ldl, l_bs, B, ldb, b_bs, nullptr, 0, 0,
-                                                                                32);
+  if (const int rc = opt_in_smem<trsm_leaf_tc_kernel<T>>(TC_SMEM)) return rc;
+  trsm_leaf_tc_kernel<T><<<dim3(4, (unsigned)batch), TC_THREADS, TC_SMEM, stream>>>(L, ldl, l_bs, B, ldb, b_bs, 32);
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();
   diag_syrk_kernel<T><<<dim3(17, (unsigned)batch), 256, 0, stream>>>(B, ldb, b_bs, D, ldd, d_bs);
@@ -669,17 +616,11 @@ static int launch_potrf_leaf(T* A, int64_t lda, int64_t a_bs, T* logdet, int32_t
   //  A two-columns-per-barrier (rank-2) variant measured the same: the leaf is bound by its dependent
   //  STS -> barrier -> LDS -> rsqrt -> DMUL -> DFMA chain, not by the barrier count or the fp64 pipe.)
   // fp32 storage keeps the round-1 register-tiled kernel (fp32 arithmetic, measured 29.6 us against 33.6 us for the
-  // recursive one, which computes in fp64); GPK_LEAF_FLAT=1 forces it for fp64 too (A/B comparisons)
-  static const bool flat = getenv("GPK_LEAF_FLAT") != nullptr;
-  if (flat || sizeof(T) == 4) {
+  // recursive one, which computes in fp64)
+  if constexpr (sizeof(T) == 4) {
     potrf_leaf_kernel<T><<<batch, 256, 0, stream>>>(A, lda, a_bs, logdet, info, pivot_base);
   } else {
-    static bool attr_set = false;
-    if (!attr_set) {
-      cudaError_t e = cudaFuncSetAttribute(potrf_leaf_rec_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, RL_SMEM);
-      if (e != cudaSuccess) return -1000 - (int)e;
-      attr_set = true;
-    }
+    if (const int rc = opt_in_smem<potrf_leaf_rec_kernel<T>>(RL_SMEM)) return rc;
     potrf_leaf_rec_kernel<T><<<batch, RL_THREADS, RL_SMEM, stream>>>(A, lda, a_bs, logdet, info, pivot_base);
   }
   GPK_COUNT_LAUNCH();
@@ -692,15 +633,9 @@ static int launch_trsm_leaf(const T* L, int64_t ldl, int64_t l_bs, T* B, int64_t
                             int32_t batch, cudaStream_t stream) {
   if (rows == 0) return 0;
   const int smem = (NB * TL_LD + NB + 2 * 64) * (int)sizeof(T);
-  auto kern = trsm_leaf_kernel<T, TRANS>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return -1000 - (int)e;
-    attr_set = true;
-  }
+  if (const int rc = opt_in_smem<trsm_leaf_kernel<T, TRANS>>(smem)) return rc;
   dim3 grid((unsigned)(rows / 64), (unsigned)batch);
-  kern<<<grid, 256, smem, stream>>>(L, ldl, l_bs, B, ldb, b_bs);
+  trsm_leaf_kernel<T, TRANS><<<grid, 256, smem, stream>>>(L, ldl, l_bs, B, ldb, b_bs);
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();
   return 0;
@@ -713,15 +648,11 @@ static int trsm_leaf_fwd(const T* L, int64_t ldl, int64_t l_bs, T* B, int64_t ld
   return launch_trsm_leaf<T, false>(L, ldl, l_bs, B, ldb, b_bs, rows, batch, stream);
 }
 
-static int64_t nb_outer() {
-  static const int64_t v = [] {
-    const char* e = getenv("GPK_NB_OUTER");
-    int64_t x = e ? atoll(e) : 512;
-    return (x >= 128 && x % 128 == 0) ? x : 512;
-  }();
-  return v;
-}
-#define NB_OUTER nb_outer()
+constexpr int64_t NB_OUTER = 512;  // outer panel width
+
+// GPK_NO_LOOKAHEAD (read at every factorisation): the look-ahead schedule on the caller's stream alone, so that
+// event-bracketed launches time single kernels (bench.py's in-situ kernel timing)
+static bool no_lookahead() { return getenv("GPK_NO_LOOKAHEAD") != nullptr; }
 
 // Side stream + events for the look-ahead (one set per process; the library is not re-entrant across host threads
 // for potrf, like the reference's global-state model -- SURVEY 8b "Ownership / threading").
@@ -776,8 +707,8 @@ static int factor_panel(T* A, int64_t lda, int64_t a_bs, int64_t R, int64_t kb, 
 }
 
 // The same factorisation with the dependency chain cut short.  The next leaf only depends on the next 128 x 128 diagonal
-// block, so `chain` runs  leaf -> diag_step (solve the 128 rows below the leaf AND update the next diagonal block, one
-// launch) -> leaf -> ...  while every other row of the block column (the rest of the panel's diagonal block and all the
+// block, so `chain` runs  leaf -> diag_step (solve the 128 rows below the leaf, then update the next diagonal block)
+// -> leaf -> ...  while every other row of the block column (the rest of the panel's diagonal block and all the
 // rows below it: the throughput work) is solved / updated on the `bulk` stream, ordered by events:
 //   bulk(j)  waits for leaf(j) (solve) and diag_step(j) (its rows are the B operand of the update);
 //   diag_step(j + 128) waits for bulk(j) (which updated the rows it solves).
@@ -912,10 +843,8 @@ int trailing_update<double>(int used, const Trailing& t, int64_t rA, int64_t rB,
 static int potrf_driver_pairs(double* A, int64_t lda, int64_t n_pad, int64_t extra_rows, double* logdet, int32_t* info,
                               cudaStream_t stream, void* ws, int32_t S, Lookahead& la) {
   auto ce = [](cudaError_t e) { return e == cudaSuccess ? 0 : -1000 - (int)e; };
-  const int64_t R = n_pad + extra_rows, P = 512;
-  // GPK_NO_LOOKAHEAD (bench.py's in-situ kernel timing): the same schedule on ONE stream, so that event-bracketed launch
-  // durations are per-kernel figures
-  const bool nola = getenv("GPK_NO_LOOKAHEAD") != nullptr;
+  const int64_t R = n_pad + extra_rows, P = NB_OUTER;
+  const bool nola = no_lookahead();  // the same schedule on ONE stream
   const cudaStream_t side = nola ? stream : la.side, bulk = nola ? stream : la.bulk;
   auto factor = [&](int64_t c0, int64_t c1) -> int {
     if (nola) return factor_panel<double>(A, lda, 0, R, c0, c1, logdet, info, 1, stream);
@@ -996,12 +925,11 @@ static int potrf_driver(T* A, int64_t lda, int64_t a_bs, int64_t n_pad, int64_t 
   } suspend(emulation());
   int rc;
   Lookahead& la = lookahead();
-  if (tr.mode == MODE_OZAKI && sizeof(T) == 8 && batch == 1 && la.ok && NB_OUTER == 512 && n_pad >= 4096 &&
-      tr.ws_bytes >= potrf_pairs_ws_bytes(R, tr.slices) && getenv("GPK_NO_PAIRS") == nullptr)
+  if (tr.mode == MODE_OZAKI && sizeof(T) == 8 && batch == 1 && la.ok && n_pad >= 4096 &&
+      tr.ws_bytes >= potrf_pairs_ws_bytes(R, tr.slices))
     return potrf_driver_pairs(reinterpret_cast<double*>(A), lda, n_pad, extra_rows, reinterpret_cast<double*>(logdet), info,
                               stream, tr.ws, tr.slices, la);
-  const bool use_la = la.ok && n_pad > 2 * NB_OUTER && getenv("GPK_NO_LOOKAHEAD") == nullptr;
-  const bool split = use_la && getenv("GPK_NO_SPLIT") == nullptr;
+  const bool use_la = la.ok && n_pad > 2 * NB_OUTER && !no_lookahead();
   auto ce = [](cudaError_t e) { return e == cudaSuccess ? 0 : -1000 - (int)e; };
 
   const int64_t ke0 = NB_OUTER < n_pad ? NB_OUTER : n_pad;
@@ -1024,7 +952,7 @@ static int potrf_driver(T* A, int64_t lda, int64_t a_bs, int64_t n_pad, int64_t 
       // they run concurrently and the short (a) no longer costs a kernel tail of its own.
       if ((rc = ce(cudaEventRecord(la.fork, stream)))) return rc;
       if ((rc = ce(cudaStreamWaitEvent(la.side, la.fork, 0)))) return rc;
-      if (split && used != MODE_TF32X3) {
+      if (used != MODE_TF32X3) {
         // (a) in two parts: the next panel's diagonal block first (the chain starts on it at once), the rows below on `bulk`
         if ((rc = ce(cudaStreamWaitEvent(la.bulk, la.fork, 0)))) return rc;
         if ((rc = trailing_update<T>(used, tr, 0, 0, W, W, K, P, P, lda, a_bs, Ckk, 1, batch, la.side))) return rc;
@@ -1033,13 +961,9 @@ static int potrf_driver(T* A, int64_t lda, int64_t a_bs, int64_t n_pad, int64_t 
           return rc;
       } else {
         if ((rc = trailing_update<T>(used, tr, 0, 0, R - ke, W, K, P, P, lda, a_bs, Ckk, 1, batch, la.side))) return rc;
-        if (split && (rc = ce(cudaStreamWaitEvent(la.bulk, la.fork, 0)))) return rc;
+        if ((rc = ce(cudaStreamWaitEvent(la.bulk, la.fork, 0)))) return rc;
       }
-      if (split) {
-        if ((rc = factor_panel_split<T>(A, lda, a_bs, R, ke, ke2, logdet, info, batch, la.side, la))) return rc;
-      } else {
-        if ((rc = factor_panel<T>(A, lda, a_bs, R, ke, ke2, logdet, info, batch, la.side))) return rc;
-      }
+      if ((rc = factor_panel_split<T>(A, lda, a_bs, R, ke, ke2, logdet, info, batch, la.side, la))) return rc;
       if ((rc = ce(cudaEventRecord(la.join, la.side)))) return rc;
       if ((rc = trailing_update<T>(used, tr, W, W, R - ke2, n_pad - ke2, K, P2, P2, lda, a_bs, A + ke2 * lda + ke2, 1, batch,
                                    stream)))
@@ -1135,7 +1059,7 @@ int gpk_debug_leaf_phase_clock(void* buf16_int64) {
   return e == cudaSuccess ? 0 : -1000 - (int)e;
 }
 int64_t gpk_potrf_oz_ws_bytes(int64_t n_pad, int64_t extra_rows, int32_t slices) {
-  const int64_t one = gpk::oz_ws_bytes(n_pad + extra_rows, gpk::nb_outer(), slices);
+  const int64_t one = gpk::oz_ws_bytes(n_pad + extra_rows, gpk::NB_OUTER, slices);
   const int64_t pairs = gpk::potrf_pairs_ws_bytes(n_pad + extra_rows, slices);  // the pair scheme (n_pad >= 4096)
   return n_pad >= 4096 && pairs > one ? pairs : one;
 }

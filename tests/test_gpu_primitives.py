@@ -87,6 +87,24 @@ def test_gemm_nt(ops, dtype, tol):
     assert (out.double() - ref).abs().max().item() < tol * 200
     out0 = ops.gemm_nt(A, Bm)
     assert (out0.double() - A.double() @ Bm.double().transpose(1, 2)).abs().max().item() < tol * 200
+    # K = 0: exactly beta C.  Called through the C ABI with the operands' own pointers: torch reports a null data pointer
+    # for a zero-width view, which the library rejects.
+    outk0 = C.clone()
+    ops.check(ops._fn("gpk_gemm_nt", dtype)(256, 384, 0, -1.5, ops._ptr(A), A.stride(1), A.stride(0), ops._ptr(Bm),
+                                            Bm.stride(1), Bm.stride(0), 0.5, ops._ptr(outk0), outk0.stride(1),
+                                            outk0.stride(0), 0, 2, ops._stream()), "gpk_gemm_nt")
+    assert torch.equal(outk0, 0.5 * C)
+    if dtype == torch.float64:
+        # lower mode over 3600 tile rows (450 groups of 8), K = 128: the fp64 tensor-core kernel, not the emulation
+        A3 = torch.randn(1, 460800, 128, device="cuda", dtype=dtype, generator=g)
+        B3 = torch.randn(1, 256, 128, device="cuda", dtype=dtype, generator=g)
+        C3 = torch.full((1, 460800, 256), float("nan"), device="cuda", dtype=dtype)
+        ops.gemm_nt(A3, B3, C3, lower=True)
+        ref = A3[0] @ B3[0].T
+        assert (C3[0, :, :128] - ref[:, :128]).abs().max().item() < tol * 200
+        assert (C3[0, 128:, 128:] - ref[128:, 128:]).abs().max().item() < tol * 200
+        assert C3[0, :128, 128:].isnan().all()  # tile (0, 1), above the diagonal, is untouched
+        del A3, B3, C3, ref
     # lower: only tiles on/below the diagonal are touched
     S = torch.randn(1, 384, 144, device="cuda", dtype=dtype, generator=g)
     C2 = torch.zeros(1, 384, 384, device="cuda", dtype=dtype)
@@ -130,6 +148,19 @@ def test_potrf_dense_vs_torch(ops, n):
     fs = ch.full_solve(rhs)
     full_ref = torch.cholesky_solve(rhs.transpose(1, 2), Lref).transpose(1, 2)
     assert (fs - full_ref).abs().max().item() < 1e-9
+
+
+def test_potrf_on_two_devices(ops):
+    """CUDA applies a kernel's opt-in to more than 48 KB of shared memory per device: a factorisation on cuda:0, then one
+    on cuda:1 in the same process (the leaf, the tensor-core TRSM and the emulated GEMM all launch above 48 KB)."""
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs two GPUs")
+    for i in range(2):
+        with torch.cuda.device(i):  # ops launches on the current device's stream
+            K = _spd(4096, seed=i)
+            ch = ops.chol_from_dense(K).check()
+            assert ch.L().device == torch.device("cuda", i)
+            assert (ch.L() - torch.linalg.cholesky(K)).abs().max().item() < 1e-10
 
 
 def test_potrf_not_pd_reports_info(ops):

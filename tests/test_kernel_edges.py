@@ -1,16 +1,12 @@
 """K1 (``csrc/kernel_matrix.cu``) at the edges of its input range and of its launch layouts.
 
 * CPU: the host model of the fast fp64 ``exp`` (``tests/_fexp_model.py``) against a correctly rounded ``exp``.
-* GPU: every path that evaluates EQ / Matern-1/2 / 3/2 / 5/2 -- the fast strip kernel, the one-tile kernel
-  (``GPK_K1_ONE_TILE=1``, read once per process: checked in a subprocess), the generic descriptor kernel, ``kernel_diag``,
-  fp32 -- at distances from 0 to 1e9 and on NaN / inf inputs, against the closed form evaluated in fp64 on direct
-  differences with the ``exp`` taken in 40-digit decimal; and the launch layouts (strips, ragged tiles, bulk-copy and
+* GPU: every path that evaluates EQ / Matern-1/2 / 3/2 / 5/2 -- the fast strip kernel, the generic descriptor kernel,
+  ``kernel_diag``, fp32 -- at distances from 0 to 1e9 and on NaN / inf inputs, against the closed form evaluated in fp64
+  on direct differences with the ``exp`` taken in 40-digit decimal; and the launch layouts (strips, ragged tiles, bulk-copy and
   plain-load staging, LOWER, padding, strided / offset outputs, misaligned inputs, batches, groups, widths) against
   NumPy, with a sentinel checking that nothing outside the written window is touched."""
 import math
-import os
-import subprocess
-import sys
 from decimal import Decimal, localcontext
 
 import numpy as np
@@ -19,7 +15,6 @@ import torch
 
 from tests._fexp_model import GUARD, TABLE, exact_exp, fast_exp, table_index
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 KINDS = ["eq", "matern12", "matern32", "matern52"]
 DISTANCES = [0.0, 1e-8, 1.0, 37.0, 38.6, 700.0, 746.0, 6819.0, 6821.0, 7000.0, 9000.0, 16383.0, 2e4, 1e5, 1e7, 2.4e7, 1e9]
 TINY64 = 2.2250738585072014e-308
@@ -230,25 +225,6 @@ def test_fast_exp_kernel_matches_host_model_bit_for_bit(ops):
     want = np.array([fast_exp(x, table=table) for x in xs])
     bad = np.flatnonzero(got != want)
     assert bad.size == 0, (D[bad[:5]], got[bad[:5]], want[bad[:5]])
-
-
-def _one_tile_child():
-    from stheno_b200 import ops
-
-    for kind in KINDS:
-        check_values(ops, kind, "fast", torch.float64)
-        check_nonfinite(ops, kind, "fast", torch.float64)
-    print("one-tile checks passed")
-
-
-@pytest.mark.gpu
-def test_values_one_tile_kernel():
-    """``GPK_K1_ONE_TILE`` is read once per process, so the one-tile kernel (which shares ``fast_factor``) is checked in a
-    child process."""
-    code = "from tests import test_kernel_edges as t; t._one_tile_child()"
-    r = subprocess.run([sys.executable, "-c", code], cwd=ROOT, env=dict(os.environ, GPK_K1_ONE_TILE="1"),
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "one-tile checks passed" in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]
 
 
 # ---------------------------------------------------------------------------------------------------------------------

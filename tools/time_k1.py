@@ -1,25 +1,26 @@
-"""K1 A/B: specialised single-factor kernel (default) vs the generic descriptor kernel (GPK_K1_GENERIC=1): agreement and time."""
+"""K1: the specialised single-factor kernel against the generic descriptor kernel, agreement and time.  The generic kernel
+runs the same kernel with a ``("one", 0)`` factor appended, which the specialised one does not take.
+python tools/time_k1.py  ->  one JSON line per kernel."""
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def child():
-    import numpy as np
+def run_variant(variant):
     import torch
 
     sys.path.insert(0, ROOT)
     from stheno_b200 import ops
 
-    out = {"variant": "generic" if os.environ.get("GPK_K1_GENERIC") else "fast"}
+    out = {"variant": variant}
     g = torch.Generator(device="cuda").manual_seed(1)
     n, d = 16384, 8
     x = torch.randn(1, 1, n, d, device="cuda", dtype=torch.float64, generator=g) / 2.0
+    extra = [("one", 0)] if variant == "generic" else []
     for kind in ("eq", "matern12", "matern32", "matern52"):
-        flat = ops.FlatKernel([(1.3, [(kind, 0)])], 1)
+        flat = ops.FlatKernel([(1.3, [(kind, 0)] + extra)], 1)
         W = torch.empty(1, n, n, device="cuda", dtype=torch.float64)
         def run():
             ops._km_launch(flat, x, x, n, n, d, ops.KM_LOWER | ops.KM_SAME | ops.KM_PAD_IDENTITY, 0.1, None, 1e-12, W, n, n * n, 1)
@@ -48,7 +49,7 @@ def child():
         out[f"{kind}_checksum"] = float(torch.tril(W[0]).sum())
     # fp32 full square
     xf = x.float()
-    flat = ops.FlatKernel([(1.0, [("eq", 0)])], 1)
+    flat = ops.FlatKernel([(1.0, [("eq", 0)] + extra)], 1)
     Wf = torch.empty(1, n, n, device="cuda", dtype=torch.float32)
     for _ in range(3):
         ops._km_launch(flat, xf, xf, n, n, d, ops.KM_SAME, 0.1, None, 1e-6, Wf, n, n * n, 1)
@@ -66,10 +67,5 @@ def child():
 
 
 if __name__ == "__main__":
-    if len(sys.argv) > 1 and sys.argv[1] == "child":
-        child()
-    else:
-        for env in ({}, {"GPK_K1_GENERIC": "1"}):
-            e = dict(os.environ, **env)
-            r = subprocess.run([sys.executable, os.path.abspath(__file__), "child"], env=e, capture_output=True, text=True)
-            print(r.stdout.strip() or r.stderr[-2000:], flush=True)
+    for variant in ("fast", "generic"):
+        run_variant(variant)

@@ -1,20 +1,20 @@
-"""Leaf Cholesky A/B: correctness against torch.linalg.cholesky and latency, recursive (default) vs the round-1 flat kernel
-(GPK_LEAF_FLAT=1).  python tools/time_leaf.py  ->  one JSON line per variant."""
+"""Leaf Cholesky: correctness against torch.linalg.cholesky and latency of the shipped leaf kernels (fp64: the recursive
+kernel, fp32: the flat register-tiled one), and whole log-pdf steps around them.  python tools/time_leaf.py  ->  one JSON
+line."""
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def child():
+def main():
     import torch
 
     sys.path.insert(0, ROOT)
     from stheno_b200 import ops
 
-    out = {"variant": "flat" if os.environ.get("GPK_LEAF_FLAT") else "recursive"}
+    out = {}
     g = torch.Generator(device="cuda").manual_seed(0)
     for dtype, tol in ((torch.float64, 1e-12), (torch.float32, 2e-5)):
         for n, batch in ((128, 1), (128, 300), (512, 1), (1024, 3), (2000, 1)):
@@ -95,10 +95,4 @@ def child():
 
 
 if __name__ == "__main__":
-    if len(sys.argv) > 1 and sys.argv[1] == "child":
-        child()
-    else:
-        for env in ({}, {"GPK_LEAF_FLAT": "1"}):
-            e = dict(os.environ, **env)
-            r = subprocess.run([sys.executable, os.path.abspath(__file__), "child"], env=e, capture_output=True, text=True)
-            print(r.stdout.strip() or r.stderr[-2000:], flush=True)
+    main()

@@ -117,6 +117,27 @@ int gpk_kernel_matrix_bwd_f32(const gpk_kernel_desc* desc_host, const float* xg,
                               int64_t n, int32_t d, const float* G, int64_t ldg, int64_t g_bstride, float* term_sum,
                               float* grad_xg, float* diag, int32_t batch, void* stream);
 
+/* Rectangular K1-backward: K_ij = k(x*_i, x_j) (m x n) for two DIFFERENT point sets (K1 without GPK_KM_SAME: Delta is
+ * [r^2 < 1e-10] with gradient 0, no symmetry factor), upstream gradient given factored:
+ *     G_ij = r_i W_ij + u_i v_j      W: [batch] x m x n (ld = ldw, batch stride w_bstride), r, u: [batch][m], v: [batch][n]
+ * W, r, u, v may each be NULL (r = NULL: scale 1; an explicit dense G is W with r = NULL; u and v come together).
+ * gdiag ([batch][m], may be NULL) adds the prior-variance term sum_i gdiag_i k(x*_i, x*_i).  Outputs, each accumulated (the
+ * caller zeroes them) and each optional (NULL: not formed):
+ *   term_sum[b][t] += sum_ij G_ij prod_f phi_f(i, j) (+ the gdiag term)        -> d loss / d coef_t
+ *   grad_xsg[g][b][i][:] += d loss / d x*^(g)_i (layout of xsg)
+ *   grad_xg[g][b][j][:] += d loss / d x^(g)_j (layout of xg; chunks of test points add up)
+ * The posterior predictions' backward (autograd.py): G* = g_mu alpha^T - 2 diag(g_var) W with W = K* K^-1. */
+int gpk_kernel_cross_bwd_f64(const gpk_kernel_desc* desc_host, const double* xsg, int64_t xsg_gstride,
+                             int64_t xs_bstride, int64_t m, const double* xg, int64_t xg_gstride, int64_t x_bstride,
+                             int64_t n, int32_t d, const double* W, int64_t ldw, int64_t w_bstride, const double* r,
+                             const double* u, const double* v, const double* gdiag, double* term_sum, double* grad_xsg,
+                             double* grad_xg, int32_t batch, void* stream);
+int gpk_kernel_cross_bwd_f32(const gpk_kernel_desc* desc_host, const float* xsg, int64_t xsg_gstride, int64_t xs_bstride,
+                             int64_t m, const float* xg, int64_t xg_gstride, int64_t x_bstride, int64_t n, int32_t d,
+                             const float* W, int64_t ldw, int64_t w_bstride, const float* r, const float* u,
+                             const float* v, const float* gdiag, float* term_sum, float* grad_xsg, float* grad_xg,
+                             int32_t batch, void* stream);
+
 /* GEMM  C = beta*C + alpha * A * B^T   (A: M x K, B: N x K, both K-contiguous; C: M x N).
  * M, N multiples of 128; K a multiple of 16; pointers 16-byte aligned; ld multiples of 2.
  * lower != 0: only tiles with (row tile >= col tile) are touched (SYRK-style trailing update, M >= N).

@@ -7,14 +7,18 @@ ANALYTIC backward (SURVEY.md section 7 step 8, section 8 row a16):
 (kernel scales, length scales through the pre-stretched inputs, inputs, noise) happens inside the K1-backward kernel
 (``csrc/kernel_matrix_bwd.cu``) so no ``n x n`` gradient tensor per hyper-parameter is ever formed.  The reference gets
 these gradients from torch autograd through ``exp`` / ``cholesky`` / ``triangular_solve``
-(``readme_example13_optimisation_torch.py:46-53``)."""
+(``readme_example13_optimisation_torch.py:46-53``).
+
+Cross-covariances ``k(x, y)``, ``k.elwise(x)`` and exact posterior predictions get analytic backwards the same way: the
+rectangular K1-backward (``gpk_kernel_cross_bwd``) contracts ``d loss / d k(x*, x)`` in factored form."""
 import ctypes
 
 import torch
 
 from . import _lib, ops
 
-__all__ = ["kernel_logpdf", "dense_logpdf", "kernel_matrix_grad"]
+__all__ = ["kernel_logpdf", "dense_logpdf", "kernel_matrix_grad", "kernel_cross_grad", "kernel_diag_grad", "exact_posterior",
+           "no_gradient"]
 
 
 def _bwd_kernel(flat, xg, G, n):
@@ -130,16 +134,258 @@ class _KernelMatrix(torch.autograd.Function):
         return term_sum[:, : len(flat.terms)].sum(0), grad_xg, None
 
 
-def kernel_matrix_grad(flat, xg):
-    """``k(x, x) [B, n, n]`` with an autograd graph to the kernel's tensor hyper-parameters and to ``xg``."""
+def coef_tensor(flat, like):
+    """The coefficients of ``flat`` as one ``[T]`` tensor on ``like``'s device, with the graph of those given as tensors."""
     raw = getattr(flat, "coef_raw", None) or [c for c, _ in flat.terms]
-    coefs = torch.stack([
-        (c if isinstance(c, torch.Tensor) else torch.tensor(float(c))).to(device=xg.device, dtype=xg.dtype).reshape(())
+    return torch.stack([
+        (c if isinstance(c, torch.Tensor) else torch.tensor(float(c))).to(device=like.device, dtype=like.dtype).reshape(())
         for c in raw
     ])
-    return _KernelMatrix.apply(coefs, xg, [fs for _, fs in flat.terms])
+
+
+def kernel_matrix_grad(flat, xg):
+    """``k(x, x) [B, n, n]`` with an autograd graph to the kernel's tensor hyper-parameters and to ``xg``."""
+    return _KernelMatrix.apply(coef_tensor(flat, xg), xg, [fs for _, fs in flat.terms])
 
 
 def kernel_logpdf(coefs, xg, noise_scalar, noise_vec, rhs_t, structure, jitter):
     """Differentiable ``logpdf`` ``[B, k]`` of ``N(0, sum_t coefs[t] prod phi(xg) + noise + jitter I)`` at ``rhs_t``."""
     return _KernelLogpdf.apply(coefs, xg, noise_scalar, noise_vec, rhs_t, structure, jitter)
+
+
+def _flat_of(coefs, structure, n_groups):
+    return ops.FlatKernel([(float(c), fs) for c, fs in zip(coefs.tolist(), structure)], n_groups)
+
+
+class _KernelCross(torch.autograd.Function):
+    """Differentiable ``k(x, y)`` for two different point sets, built by K1; backward = the rectangular K1-backward."""
+
+    @staticmethod
+    def forward(ctx, coefs, xsg, xg, structure):
+        flat = _flat_of(coefs, structure, xsg.shape[0])
+        ctx.flat, ctx.xsg, ctx.xg = flat, xsg.detach().contiguous(), xg.detach().contiguous()
+        return ops.kernel_matrix(flat, ctx.xsg, ctx.xg, same=False)
+
+    @staticmethod
+    def backward(ctx, G):
+        flat, xsg, xg = ctx.flat, ctx.xsg, ctx.xg
+        nig = ctx.needs_input_grad
+        ts = torch.zeros(xsg.shape[1], _lib.GPK_MAX_TERMS, dtype=xsg.dtype, device=xsg.device) if nig[0] else None
+        gxs = torch.zeros_like(xsg) if nig[1] else None
+        gx = torch.zeros_like(xg) if nig[2] else None
+        ops.kernel_cross_bwd(flat, xsg, xg, W=G.contiguous(), term_sum=ts, grad_xsg=gxs, grad_xg=gx)
+        return None if ts is None else ts[:, : len(flat.terms)].sum(0), gxs, gx, None
+
+
+def kernel_cross_grad(flat, xsg, xg):
+    """``k(x, y) [B, m, n]`` (``x is not y``) with an autograd graph to the kernel's tensor hyper-parameters, ``xsg`` and
+    ``xg``."""
+    return _KernelCross.apply(coef_tensor(flat, xsg), xsg, xg, [fs for _, fs in flat.terms])
+
+
+class _KernelDiag(torch.autograd.Function):
+    """Differentiable ``k.elwise(x)`` (same points); the backward is the prior-variance term of the rectangular K1-backward."""
+
+    @staticmethod
+    def forward(ctx, coefs, xg, structure):
+        flat = _flat_of(coefs, structure, xg.shape[0])
+        ctx.flat, ctx.xg = flat, xg.detach().contiguous()
+        return ops.kernel_diag(flat, ctx.xg)
+
+    @staticmethod
+    def backward(ctx, g):
+        flat, xg = ctx.flat, ctx.xg
+        nig = ctx.needs_input_grad
+        ts = torch.zeros(xg.shape[1], _lib.GPK_MAX_TERMS, dtype=xg.dtype, device=xg.device) if nig[0] else None
+        gx = torch.zeros_like(xg) if nig[1] else None
+        ops.kernel_cross_bwd(flat, xg, xg, gdiag=g.contiguous(), term_sum=ts, grad_xsg=gx)
+        return None if ts is None else ts[:, : len(flat.terms)].sum(0), gx, None
+
+
+def kernel_diag_grad(flat, xg):
+    """``k.elwise(x) [B, n]`` with an autograd graph to the kernel's tensor hyper-parameters and to ``xg``."""
+    return _KernelDiag.apply(coef_tensor(flat, xg), xg, [fs for _, fs in flat.terms])
+
+
+class _NoGradient(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, route, value, *inputs):
+        ctx.route = route
+        return value.detach().clone()
+
+    @staticmethod
+    def backward(ctx, *grads):
+        raise NotImplementedError(f"gradients through {ctx.route} are not implemented")
+
+
+def no_gradient(route, value, inputs):
+    """``value`` unchanged, attached to ``inputs`` (the tensors that require grad and feed it) by a node whose backward raises
+    ``NotImplementedError`` naming ``route``: reading the value works, a ``backward()`` that would return wrong gradients
+    through a raw-pointer kernel does not."""
+    return _NoGradient.apply(route, value, *inputs)
+
+
+# ---- exact posterior predictions --------------------------------------------------------------------------------------
+#
+# K = k(x, x) + noise + eps I = L L^T,  alpha = K^-1 ybar,  K* = k(x*, x),  V = K* L^-T,  W = V L^-1 = K* K^-1.
+# Outputs (per problem): dot = K* alpha,  sq = rowsum(V o V),  C = P - V V^T (P = k(x*, x*), lower triangle mirrored).
+# With upstream gradients a (dot), s (sq), gC (C), H = -(gC + gC^T) / 2 and D = diag(s) + H:
+#   d/dK*  = a alpha^T + 2 D W                         (rectangular K1-backward, factored: no m x n buffer for D = 0)
+#   d/dK   = -(beta alpha^T + alpha beta^T) / 2 - W^T D W,   beta = W^T a = K^-1 K*^T a   (square K1-backward)
+#   d/dybar = beta,   d/dP = the lower-mirrored gC
+class PosteriorSpec:
+    """What one exact-posterior evaluation needs beyond its tensor inputs: the factor ``ch`` of ``K_x``, ``K_x``'s flat
+    kernel, the cross kernel ``flat_c``, ``half_y = L^-1 ybar`` padded ``[B, n_pad]`` (None without a mean output), and
+    ``fwd()``, which runs the launches of the no-grad path and returns ``(dot, sq, cov)`` (None for outputs not formed)."""
+
+    def __init__(self, ch, flat_x, flat_c, half_y, fwd, chunk=4096):
+        self.ch, self.flat_x, self.flat_c, self.half_y, self.fwd, self.chunk = ch, flat_x, flat_c, half_y, fwd, chunk
+
+
+class _ExactPosterior(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, spec, coefs_x, xg_x, noise_s, noise_v, ybar, coefs_c, xsg, zg, P):
+        ctx.set_materialize_grads(False)
+        ctx.spec = spec
+        ctx.xg_x, ctx.xsg, ctx.zg = xg_x.detach().contiguous(), xsg.detach().contiguous(), zg.detach().contiguous()
+        ctx.ybar_shape = None if ybar is None else ybar.shape
+        ctx.P_shape = None if P is None else P.shape
+        outs = []
+        for t in spec.fwd():
+            if t is None:
+                t = xsg.new_empty(0)
+                ctx.mark_non_differentiable(t)
+            outs.append(t)
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, g_dot, g_sq, g_cov):
+        return (None,) + _posterior_backward(ctx, g_dot, g_sq, g_cov)
+
+
+def exact_posterior(spec, coefs_x, xg_x, noise_s, noise_v, ybar, coefs_c, xsg, zg, P=None):
+    """``(dot, sq, cov)`` of the exact posterior as ``spec.fwd()`` computes them (an empty tensor for those not formed),
+    differentiable w.r.t. ``K_x``'s coefficients, inputs ``xg_x`` and noise, ``ybar [B, n]``, the cross kernel's coefficients,
+    the test points ``xsg``, the data points ``zg`` (both stretched by the cross kernel's length scales) and the prior
+    covariance ``P`` of ``cov``."""
+    return _ExactPosterior.apply(spec, coefs_x, xg_x, noise_s, noise_v, ybar, coefs_c, xsg, zg, P)
+
+
+def _posterior_backward(ctx, a, s, gc):
+    spec, ch = ctx.spec, ctx.spec.ch
+    flat_c, flat_x = spec.flat_c, spec.flat_x
+    xsg, zg, xg_x = ctx.xsg, ctx.zg, ctx.xg_x
+    _, want_coefs_x, want_xg_x, want_ns, want_nv, want_y, want_coefs_c, want_xs, want_z, want_P = ctx.needs_input_grad
+    Bn, n, n_pad, m = ch.batch, ch.n, ch.n_pad, xsg.shape[2]
+    dt, dev = ch.dtype, ch.device
+    want_K = want_coefs_x or want_xg_x or want_ns or want_nv
+    want_cross = want_coefs_c or want_xs or want_z
+    a = None if a is None else a.reshape(Bn, m)
+    s = None if s is None else s.reshape(Bn, m)
+    need_W = (s is not None or gc is not None) and (want_cross or want_K)
+    need_beta = a is not None and (want_K or want_y)
+
+    # alpha = K^-1 ybar and beta = K^-1 K*^T a: one-row solves in one 128-row buffer
+    alpha = beta = None
+    if a is not None and (want_cross or want_K or want_y):
+        buf = ch.new_rows(2)
+        if need_beta:
+            buf[:, 1, :n] = _kt_dot(flat_c, zg, xsg, a)
+            ch.solve_rows_(buf)
+        buf[:, 0, :] = spec.half_y
+        ch.solve_rows_t_(buf)
+        alpha, beta = buf[:, 0, :n], buf[:, 1, :n]
+
+    ts_c = torch.zeros(Bn, _lib.GPK_MAX_TERMS, dtype=dt, device=dev) if want_coefs_c else None
+    g_xs = torch.zeros_like(xsg) if want_xs else None
+    g_z = torch.zeros_like(zg) if want_z else None
+    GK = torch.zeros(Bn, n_pad, n_pad, dtype=dt, device=dev) if want_K else None
+    cross_out = dict(term_sum=ts_c, grad_xg=g_z)
+    fac = dict(u=a, v=alpha) if a is not None else {}
+
+    if not need_W:
+        if want_cross and a is not None:
+            ops.kernel_cross_bwd(flat_c, xsg, zg, grad_xsg=g_xs, **fac, **cross_out)
+    elif gc is None:
+        # marginals: walk the test points in chunks, as the forward does; D = diag(s)
+        for c0 in range(0, m, spec.chunk):
+            c1 = min(m, c0 + spec.chunk)
+            xs_c = xsg[:, :, c0:c1].contiguous()
+            Wc = _solved_rows(ch, flat_c, xs_c, zg)
+            s_c = s[:, c0:c1]
+            if want_cross:
+                gxs_c = torch.zeros_like(xs_c) if want_xs else None
+                fac_c = dict(u=a[:, c0:c1], v=alpha) if a is not None else {}
+                ops.kernel_cross_bwd(flat_c, xs_c, zg, W=Wc, r=2.0 * s_c, grad_xsg=gxs_c, **fac_c, **cross_out)
+                if want_xs:
+                    g_xs[:, :, c0:c1] = gxs_c
+            if want_K:  # GK -= W_c^T diag(s_c) W_c
+                cp = Wc.shape[1]
+                Wt = ops.transpose(Wc, cp, n_pad)
+                del Wc
+                sp = torch.zeros(Bn, 1, cp, dtype=dt, device=dev)
+                sp[:, 0, : c1 - c0] = s_c
+                ops.gemm_nt(Wt * sp, Wt, GK, alpha=-1.0, beta=1.0, lower=True)
+    else:
+        # full covariance: every test point at once (the forward holds them all too); D = diag(s) + H
+        W = _solved_rows(ch, flat_c, xsg, zg)
+        mp = W.shape[1]
+        D2 = torch.zeros(Bn, mp, mp, dtype=dt, device=dev)
+        D2[:, :m, :m] = -(gc.reshape(Bn, m, m) + gc.reshape(Bn, m, m).transpose(1, 2))
+        if s is not None:
+            D2.diagonal(dim1=1, dim2=2)[:, :m] += 2.0 * s
+        Wt = ops.transpose(W, mp, n_pad)
+        Y = ops.gemm_nt(D2, Wt)  # 2 D W
+        del D2
+        if want_cross:
+            ops.kernel_cross_bwd(flat_c, xsg, zg, W=Y, grad_xsg=g_xs, **fac, **cross_out)
+        if want_K:
+            Yt = ops.transpose(Y, mp, n_pad)
+            ops.gemm_nt(Wt, Yt, GK, alpha=-0.5, beta=1.0, lower=True)
+
+    grad_coefs_x = grad_xg_x = grad_ns = grad_nv = None
+    if want_K:
+        if a is not None:  # GK -= (beta alpha^T + alpha beta^T) / 2
+            A2 = torch.zeros(Bn, n_pad, 16, dtype=dt, device=dev)
+            B2 = torch.zeros(Bn, n_pad, 16, dtype=dt, device=dev)
+            A2[:, :n, 0], A2[:, :n, 1] = beta, alpha
+            B2[:, :n, 0], B2[:, :n, 1] = alpha, beta
+            ops.gemm_nt(A2, B2, GK, alpha=-0.5, beta=1.0, lower=True)
+        ops.symmetrize_(GK, n_pad)
+        term_sum, grad_xg_x, diag = _bwd_kernel(flat_x, xg_x, GK, n)
+        del GK
+        grad_coefs_x = term_sum[:, : len(flat_x.terms)].sum(0) if want_coefs_x else None
+        grad_xg_x = grad_xg_x if want_xg_x else None
+        grad_ns = diag.sum() if want_ns else None
+        grad_nv = diag if want_nv else None
+    grad_y = beta.reshape(ctx.ybar_shape) if (want_y and beta is not None) else None
+    grad_coefs_c = ts_c[:, : len(flat_c.terms)].sum(0) if want_coefs_c else None
+    grad_P = None
+    if want_P:
+        g = gc.reshape(-1, m, m)
+        grad_P = (torch.tril(g + g.transpose(1, 2), -1) + torch.diag_embed(torch.diagonal(g, dim1=1, dim2=2)))
+        grad_P = grad_P.reshape(ctx.P_shape)
+    return grad_coefs_x, grad_xg_x, grad_ns, grad_nv, grad_y, grad_coefs_c, g_xs, g_z, grad_P
+
+
+def _solved_rows(ch, flat_c, xs_c, zg):
+    """``W_c = k(x*_c, x) K^-1`` as padded rows ``[B, c_pad, n_pad]``: K1 rows, then both triangular solves in place."""
+    Wc = ops.kernel_rows_padded(flat_c, xs_c, zg, ch)
+    ch.solve_rows_(Wc)
+    ch.solve_many_rows_t_(Wc)
+    return Wc
+
+
+def _kt_dot(flat_c, zg, xsg, a, max_bytes=32 << 20):
+    """``u = k(x*, x)^T a`` ``[B, n]``: K1 builds ``k(x, x*_c)`` for chunks of test points small enough that a chunk takes
+    at most ``max_bytes``, and one row reduction per chunk contracts it with ``a_c``."""
+    Bn, n, m = zg.shape[1], zg.shape[2], xsg.shape[2]
+    c = max(128, (max_bytes // (n * zg.element_size())) // 128 * 128)
+    u = torch.zeros(Bn, n, dtype=zg.dtype, device=zg.device)
+    for c0 in range(0, m, c):
+        c1 = min(m, c0 + c)
+        Kt = ops.kernel_matrix(flat_c, zg, xsg[:, :, c0:c1].contiguous(), same=False)  # [B, n, c]
+        dot, _ = ops.row_dot_sq(Kt, n, c1 - c0, a[:, c0:c1], want_sq=False)
+        u += dot
+        del Kt
+    return u

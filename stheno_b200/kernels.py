@@ -266,7 +266,12 @@ class Kernel:
             return torch.zeros(x.batch_shape + (x.n, y.n), dtype=x.t.dtype, device=x.t.device)
         xg = x.scaled(scales)
         yg = xg if same else y.scaled(scales)
-        K = ops.kernel_matrix(flat, xg, None if same else yg, same=same)
+        if torch.is_grad_enabled() and (flat.coef_raw is not None or xg.requires_grad or yg.requires_grad):
+            from .autograd import kernel_cross_grad, kernel_matrix_grad
+
+            K = kernel_matrix_grad(flat, xg) if same else kernel_cross_grad(flat, xg, yg)
+        else:
+            K = ops.kernel_matrix(flat, xg, None if same else yg, same=same)
         return K.reshape(x.batch_shape + (x.n, y.n))
 
     def _elwise_dev(self, x, y, same):
@@ -277,7 +282,16 @@ class Kernel:
             return torch.zeros(x.batch_shape + (x.n, 1), dtype=x.t.dtype, device=x.t.device)
         xg = x.scaled(scales)
         yg = xg if same else y.scaled(scales)
-        k = ops.kernel_diag(flat, xg, None if same else yg, same=same)
+        if torch.is_grad_enabled() and (flat.coef_raw is not None or xg.requires_grad or yg.requires_grad):
+            from .autograd import kernel_diag_grad, no_gradient
+
+            if same:
+                k = kernel_diag_grad(flat, xg)
+            else:
+                k = no_gradient("k.elwise(x, y) with x is not y", ops.kernel_diag(flat, xg, yg, same=False),
+                                _grad_tensors(self, x, y))
+        else:
+            k = ops.kernel_diag(flat, xg, None if same else yg, same=same)
         return k.reshape(x.batch_shape + (x.n, 1))
 
     def _matrix(self, x, y, same):
@@ -912,6 +926,79 @@ def _cross_rows(k_zi, z, x, ch):
     return buf, K3.shape[2]
 
 
+def _grad_tensors(*objs):
+    """The tensors that require grad reachable from the kernels, means, inputs, matrices and tensors ``objs`` (empty when
+    grad mode is off): what a posterior prediction depends on through raw-pointer kernels."""
+    from .model.fdd import FDD
+
+    out, seen = [], set()
+    if not torch.is_grad_enabled():
+        return out
+
+    def walk(o):
+        if o is None or id(o) in seen:
+            return
+        seen.add(id(o))
+        if isinstance(o, torch.Tensor):
+            if o.requires_grad:
+                out.append(o)
+        elif isinstance(o, (list, tuple)):
+            for v in o:
+                walk(v)
+        elif isinstance(o, Input):
+            walk(o.t)
+        elif isinstance(o, FDD):
+            walk(o.x)
+        elif isinstance(o, M.KernelDense):
+            walk([getattr(o.flat, "coef_raw", None), o.xg, o.noise_t, o.noise_vec])
+        elif isinstance(o, (Kernel, Mean, InputMap, M.AbstractMatrix)):
+            for k, v in vars(o).items():
+                if k not in ("_chol", "_b"):
+                    walk(v)
+
+    for o in objs:
+        walk(o)
+    return out
+
+
+def _exact_route(K_z, k_zi, z, x, *others):
+    """How a posterior prediction at ``x`` is evaluated: None when no gradient is requested (the raw-pointer path), else
+    ``(args, tensors)`` -- ``args`` the inputs of :func:`autograd.exact_posterior` when the posterior is covered (exact
+    observations with a symbolic ``K_z``, a symmetric cross kernel that flattens to one descriptor, single-output inputs of
+    the factor's batch), None when it is not."""
+    ts = _grad_tensors(K_z, k_zi, z, x, *others)
+    if not ts:
+        return None
+    if not isinstance(K_z, M.KernelDense) or _is_multi(x) or _is_multi(z) or not k_zi.symmetric:
+        return None, ts
+    flat, scales = k_zi._flat()
+    if flat is None or not flat.terms:
+        return None, ts
+    xi, zi = as_input(x), as_input(z)
+    xsg, zg = xi.scaled(scales), zi.scaled(scales)
+    if xsg.shape[1] != K_z.xg.shape[1] or zg.shape[1] != K_z.xg.shape[1] or zg.shape[2] != K_z.n:
+        return None, ts
+    from .autograd import coef_tensor
+
+    coefs_x, ns = K_z.grad_params()
+    return (flat, [coefs_x, K_z.xg, ns, K_z.noise_vec, coef_tensor(flat, xsg), xsg, zg]), ts
+
+
+def _exact_posterior(K_z, route, ybar, fwd, half_y=None, P=None):
+    """``(dot, sq, cov)`` from ``fwd()`` with the analytic backward of ``autograd.exact_posterior``."""
+    from .autograd import PosteriorSpec, exact_posterior
+
+    flat, (coefs_x, xg_x, ns, nv, coefs_c, xsg, zg) = route
+    spec = PosteriorSpec(K_z.chol(), K_z.flat, flat, half_y, fwd)
+    return exact_posterior(spec, coefs_x, xg_x, ns, nv, ybar, coefs_c, xsg, zg, P)
+
+
+def _uncovered(route, value, ts):
+    from .autograd import no_gradient
+
+    return no_gradient(route, value, ts)
+
+
 class PosteriorKernel(Kernel):
     """``k_ij(x, y) - k_zi(z, x)^T K_z^-1 k_zj(z, y)`` (``stheno/model/observations.py:148-154``)."""
 
@@ -928,8 +1015,35 @@ class PosteriorKernel(Kernel):
 
     def _pairwise_any(self, x, y, same):
         org = _origin_of_input(x)
-        Vx, mx = self._half(self.k_zi, x)
         same_half = same and (self.k_zi is self.k_zj)
+        route = _exact_route(self.K_z, self.k_zi, self.z, x, self.k_zj, None if same else y)
+        if route is None or route[0] is None:
+            C = self._pairwise_raw(x, y, same, same_half)
+            if route is not None:
+                C = _uncovered(f"the posterior covariance of a {_route_name(self)}", C, route[1] + [C])
+            return M.Dense(C, org)
+        if not same_half:
+            C = self._pairwise_raw(x, y, same, same_half)
+            return M.Dense(_uncovered("a posterior cross-covariance between different inputs or processes", C,
+                                      route[1] + [C]), org)
+        prior = M.dense(pairwise(self.k_ij, x))
+        _, _, C = _exact_posterior(self.K_z, route[0], None, lambda: (None, None, self._cov_lower(x, prior)), P=prior)
+        return M.Dense(C, org)
+
+    def _cov_lower(self, x, prior, V=None, m=None):
+        """``prior - V V^T`` from the lower triangle of the product, mirrored (``V``: the solved rows at ``x``).  The copy of
+        ``prior`` keeps its graph: when nothing behind ``V`` requires grad, the result's gradient is the prior's alone."""
+        if V is None:
+            V, m = self._half(self.k_zi, x)
+        P3, bs = batch_flatten(prior, 2)
+        C = torch.zeros(P3.shape[0], V.shape[1], V.shape[1], dtype=P3.dtype, device=P3.device)
+        C[:, :m, :m] = P3
+        ops.gemm_nt(V, V, C, alpha=-1.0, beta=1.0, lower=True)
+        ops.symmetrize_(C, m)
+        return C[:, :m, :m].reshape(bs + (m, m))
+
+    def _pairwise_raw(self, x, y, same, same_half):
+        Vx, mx = self._half(self.k_zi, x)
         Vy, my = (Vx, mx) if same_half else self._half(self.k_zj, x if same else y)
         prior = M.dense(pairwise(self.k_ij, x, None if same else y))
         P3, bs = batch_flatten(prior, 2)
@@ -938,19 +1052,29 @@ class PosteriorKernel(Kernel):
         ops.gemm_nt(Vx, Vy, C, alpha=-1.0, beta=1.0, lower=same_half)
         if same_half:
             ops.symmetrize_(C, mx)
-        return M.Dense(C[:, :mx, :my].reshape(bs + (mx, my)), org)
+        return C[:, :mx, :my].reshape(bs + (mx, my))
 
     def _elwise_any(self, x, y, same):
-        Vx, mx = self._half(self.k_zi, x)
         same_half = same and (self.k_zi is self.k_zj)
         prior = _elwise_any(self.k_ij, x, y, same)
-        if same_half:
-            _, sq = ops.row_dot_sq(Vx, mx, Vx.shape[2], None)
-            corr = sq
+        route = _exact_route(self.K_z, self.k_zi, self.z, x, self.k_zj, None if same else y)
+        if route is not None and route[0] is not None and same_half:
+            _, corr, _ = _exact_posterior(self.K_z, route[0], None, lambda: (None, self._sq(x), None))
         else:
-            Vy, _ = self._half(self.k_zj, x if same else y)
-            corr = (Vx[:, :mx] * Vy[:, :mx]).sum(-1)
+            corr = self._sq(x) if same_half else self._corr(x, y, same)
+            if route is not None:
+                name = "a " + _route_name(self) if route[0] is None else "a cross-covariance between different inputs"
+                corr = _uncovered(f"the posterior variance of {name}", corr, route[1])
         return prior - corr.reshape(prior.shape[:-1]).unsqueeze(-1)
+
+    def _sq(self, x):
+        Vx, mx = self._half(self.k_zi, x)
+        return ops.row_dot_sq(Vx, mx, Vx.shape[2], None)[1]
+
+    def _corr(self, x, y, same):
+        Vx, mx = self._half(self.k_zi, x)
+        Vy, _ = self._half(self.k_zj, x if same else y)
+        return (Vx[:, :mx] * Vy[:, :mx]).sum(-1)
 
     def _matrix(self, x, y, same):
         return self._pairwise_any(x, y, same)
@@ -986,14 +1110,18 @@ class SubspaceKernel(Kernel):
         Vy, my = (Vx, mx) if same_half else self._half(self.k_zj, x if same else y)
         C = ops.gemm_nt(Vx, Vy, lower=False)
         bs = _batch_shape_of_input(x)
-        return M.Dense(C[:, :mx, :my].reshape(bs + (mx, my)), org)
+        return M.Dense(self._no_grad(C[:, :mx, :my].reshape(bs + (mx, my)), x, y), org)
 
     def _elwise_any(self, x, y, same):
         Vx, mx = self._half(self.k_zi, x)
         same_half = same and (self.k_zi is self.k_zj)
         Vy = Vx if same_half else self._half(self.k_zj, x if same else y)[0]
         out = (Vx[:, :mx] * Vy[:, :mx]).sum(-1)
-        return out.reshape(_batch_shape_of_input(x) + (mx, 1))
+        return self._no_grad(out.reshape(_batch_shape_of_input(x) + (mx, 1)), x, y)
+
+    def _no_grad(self, value, x, y):
+        ts = _grad_tensors(self.A, self.k_zi, self.k_zj, self.z, x, y)
+        return _uncovered("a sparse (pseudo-observation) posterior", value, ts) if ts else value
 
     def _matrix(self, x, y, same):
         return self._pairwise_any(x, y, same)
@@ -1274,20 +1402,50 @@ class PosteriorMean(Mean):
             self._b = b
         return self._b
 
-    def _dev_any(self, x, V=None, m=None):
+    def _dot(self, x, V=None, m=None):
+        """``k(x, z) K_z^-1 (y - m_z(z))`` ``[B, m]`` (``V``: the solved rows at ``x`` when already formed)."""
         ch = self.K_z.chol()
         if V is None:
             V, m = _cross_rows(self.k_zi, self.z, x, ch)
             ch.solve_rows_(V)
-        dot, _ = ops.row_dot_sq(V, m, ch.n_pad, self._half_y(), want_sq=False)
-        prior = self.m_i.dev(x)
-        return prior + dot.reshape(prior.shape[:-1]).unsqueeze(-1)
+        return ops.row_dot_sq(V, m, ch.n_pad, self._half_y(), want_sq=False)[0]
+
+    def _ybar(self):
+        """``y - m_z(z)`` as ``[B, n]`` (with its graph)."""
+        d3, _ = batch_flatten(self.y - self.m_z.dev(self.z), 2)
+        return d3[..., 0]
+
+    def _route(self, x):
+        # y - m_z(z) itself: a mean given as a user function hides its parameters in a closure
+        return _exact_route(self.K_z, self.k_zi, self.z, x, self.y, self._ybar() if torch.is_grad_enabled() else None)
 
     def dev(self, x):
-        return self._dev_any(x)
+        prior = self.m_i.dev(x)
+        route = self._route(x)
+        if route is None:
+            dot = self._dot(x)
+        elif route[0] is None:
+            dot = _uncovered(f"the posterior mean of a {_route_name(self)}", self._dot(x), route[1])
+        else:
+            dot, _, _ = _exact_posterior(self.K_z, route[0], self._ybar(), lambda: (self._dot(x), None, None),
+                                         half_y=self._half_y())
+        return prior + dot.reshape(prior.shape[:-1]).unsqueeze(-1)
 
     def render(self):
         return "PosteriorMean()"
+
+
+def _route_name(post):
+    """The posterior kind named by the error of an uncovered gradient route."""
+    from .model.fdd import FDD
+
+    K_z = post.K_z
+    if isinstance(K_z, M.BlockDense) or isinstance(post.z, (tuple, FDD)):
+        return "multi-output posterior"
+    if isinstance(K_z, M.KernelDense):
+        return "posterior whose cross kernel is not one flat kernel expression (input maps, derivatives, periodic, " \
+               "function-scaled, reversed) or whose inputs are multi-output or of another batch"
+    return "sparse (pseudo-observation) or non-kernel posterior"
 
 
 def _shared_posterior(mean, kernel):
@@ -1305,15 +1463,22 @@ def mean_var(mean, kernel, x):
     """``mlkernels.mean_var``: mean ``[..., n, 1]`` (device) and variance (matrix), sharing ``L^-1 k(z, x)`` between
     the two for an exact posterior (``stheno/model/fdd.py:68-70``)."""
     if _shared_posterior(mean, kernel) and not _is_multi(x):
-        V, m = kernel._half(kernel.k_zi, x)
-        mu = mean._dev_any(x, V, m)
+        prior_m = mean.m_i.dev(x)
         prior = M.dense(pairwise(kernel.k_ij, x))
-        P3, bs = batch_flatten(prior, 2)
-        C = torch.zeros(P3.shape[0], V.shape[1], V.shape[1], dtype=P3.dtype, device=P3.device)
-        C[:, :m, :m] = P3
-        ops.gemm_nt(V, V, C, alpha=-1.0, beta=1.0, lower=True)
-        ops.symmetrize_(C, m)
-        return mu, M.Dense(C[:, :m, :m].reshape(bs + (m, m)), _origin_of_input(x))
+        route = mean._route(x)
+        if route is not None and route[0] is None:
+            return mean.dev(x), pairwise(kernel, x)  # each raises on backward
+
+        def fwd():
+            V, m = kernel._half(kernel.k_zi, x)
+            return mean._dot(x, V, m), None, kernel._cov_lower(x, prior, V, m)
+
+        if route is None:
+            dot, _, C = fwd()
+        else:
+            dot, _, C = _exact_posterior(mean.K_z, route[0], mean._ybar(), fwd, half_y=mean._half_y(), P=prior)
+        mu = prior_m + dot.reshape(prior_m.shape[:-1]).unsqueeze(-1)
+        return mu, M.Dense(C, _origin_of_input(x))
     return mean.dev(x), pairwise(kernel, x)
 
 
@@ -1329,11 +1494,22 @@ def mean_var_diag(mean, kernel, x):
         if ch.batch == 1 and not _is_multi(kernel.z) and kernel.k_zi.symmetric:
             flat, scales = kernel.k_zi._flat()
         xi, zi = as_input(x), (as_input(kernel.z) if flat is not None else None)
-        if flat is not None and flat.terms and not xi.batch_shape and not zi.batch_shape:
-            # K3 in ONE call: kernel rows -> tensor-core solve -> both reductions, test points streamed through a bounded buffer
-            dot, sq = ops.posterior_marginals(flat, xi.scaled(scales), zi.scaled(scales), ch, mean._half_y()[0])
-        else:
+
+        def fwd():
+            if flat is not None and flat.terms and not xi.batch_shape and not zi.batch_shape:
+                # K3 in ONE call: kernel rows -> tensor-core solve -> both reductions, test points streamed through a
+                # bounded buffer
+                return ops.posterior_marginals(flat, xi.scaled(scales), zi.scaled(scales), ch, mean._half_y()[0]) + (None,)
             V, m = kernel._half(kernel.k_zi, x)
-            dot, sq = ops.row_dot_sq(V, m, ch.n_pad, mean._half_y())
+            return ops.row_dot_sq(V, m, ch.n_pad, mean._half_y()) + (None,)
+
+        route = mean._route(x)
+        if route is None:
+            dot, sq, _ = fwd()
+        elif route[0] is None:
+            dot, sq, _ = fwd()
+            dot, sq = (_uncovered(f"the posterior marginals of a {_route_name(mean)}", t, route[1]) for t in (dot, sq))
+        else:
+            dot, sq, _ = _exact_posterior(mean.K_z, route[0], mean._ybar(), fwd, half_y=mean._half_y())
         return prior_m + dot.reshape(shp).unsqueeze(-1), prior_v - sq.reshape(shp).unsqueeze(-1)
     return mean.dev(x), _elwise_any(kernel, x, None, True)

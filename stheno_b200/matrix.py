@@ -229,17 +229,19 @@ class KernelDense(Dense):
         the right-hand sides."""
         from .autograd import kernel_logpdf
 
-        raw = getattr(self.flat, "coef_raw", None) or [c for c, _ in self.flat.terms]
-        coefs = torch.stack([
-            (c if isinstance(c, torch.Tensor) else torch.tensor(float(c))).to(device=self.xg.device, dtype=self.xg.dtype).reshape(())
-            for c in raw
-        ])
+        coefs, ns = self.grad_params()
+        structure = [fs for _, fs in self.flat.terms]
+        return kernel_logpdf(coefs, self.xg, ns, self.noise_vec, rhs_t, structure, _B.epsilon)
+
+    def grad_params(self):
+        """``(coefs [T], scalar noise [])`` as tensors carrying the graph of those given as tensors that require grad."""
+        from .autograd import coef_tensor
+
         if self.noise_t is not None:
             ns = self.noise_t.to(device=self.xg.device, dtype=self.xg.dtype).reshape(())
         else:
             ns = torch.tensor(self.noise_scalar, device=self.xg.device, dtype=self.xg.dtype)
-        structure = [fs for _, fs in self.flat.terms]
-        return kernel_logpdf(coefs, self.xg, ns, self.noise_vec, rhs_t, structure, _B.epsilon)
+        return coef_tensor(self.flat, self.xg), ns
 
 
 class BlockDense(Dense):

@@ -166,6 +166,33 @@ def kernel_diag(flat, xg, yg=None, *, same=None):
     return out
 
 
+def kernel_cross_bwd(flat, xsg, xg, *, W=None, r=None, u=None, v=None, gdiag=None, term_sum=None, grad_xsg=None,
+                     grad_xg=None):
+    """Rectangular K1-backward (``gpk_kernel_cross_bwd``) of ``K = k(x*, x)`` ``[B, m, n]`` for the upstream gradient
+    ``G_ij = r_i W_ij + u_i v_j`` (+ ``gdiag_i`` on ``k(x*_i, x*_i)``).  ``W``: ``[B, >= m, ldw]`` with a unit inner stride;
+    ``r``, ``u``, ``gdiag``: ``[B, m]``; ``v``: ``[B, n]``.  The outputs ``term_sum [B, GPK_MAX_TERMS]``, ``grad_xsg`` (like
+    ``xsg``) and ``grad_xg`` (like ``xg``) are accumulated into; pass the ones wanted (None: not formed)."""
+    _check_groups(xsg, flat)
+    _check_groups(xg, flat)
+    _require_cuda(xsg, xg, W, r, u, v, gdiag, term_sum, grad_xsg, grad_xg)
+    for t, like in ((grad_xsg, xsg), (grad_xg, xg)):
+        if t is not None and (t.shape != like.shape or not t.is_contiguous()):
+            raise ValueError("kernel_cross_bwd: gradient outputs must be contiguous and shaped like their inputs")
+    xsg, xg = xsg.contiguous(), xg.contiguous()
+    B, m, d = xsg.shape[1], xsg.shape[2], xsg.shape[3]
+    n = xg.shape[2]
+    if W is not None and W.stride(2) != 1:
+        W = W.contiguous()
+    r, u, v, gdiag = [None if t is None else t.contiguous() for t in (r, u, v, gdiag)]
+    desc = flat.desc()
+    rc = _fn("gpk_kernel_cross_bwd", xsg.dtype)(
+        ctypes.byref(desc), _ptr(xsg), xsg.stride(0), xsg.stride(1), m, _ptr(xg), xg.stride(0), xg.stride(1), n, d,
+        _ptr(W), (W.stride(1) if W is not None else 0), (W.stride(0) if W is not None else 0), _ptr(r), _ptr(u), _ptr(v),
+        _ptr(gdiag), _ptr(term_sum), _ptr(grad_xsg), _ptr(grad_xg), B, _stream(),
+    )
+    check(rc, "gpk_kernel_cross_bwd")
+
+
 def gemm_nt(A, Bm, C=None, *, alpha=1.0, beta=0.0, lower=False):
     """``C = beta * C + alpha * A @ Bm^T`` on padded ``[B, M, K]`` / ``[B, N, K]`` tensors (views with a unit inner
     stride are fine).  Returns ``C``."""
@@ -330,6 +357,35 @@ class Chol:
         )
         check(rc, "gpk_trsm_right_t")
         return Bt
+
+    def solve_many_rows_t_(self, Bt, leaf=1024, panel=1024):
+        """:meth:`solve_rows_t_` for many rows (a chunk of test points).  ``gpk_trsm_right_t`` is a CUDA-core backward
+        substitution that re-reads ``L`` for every row; here ``L`` is split recursively, the trailing block is solved first
+        and its product with the off-diagonal block is subtracted on the tensor-core GEMM (through transposed copies of
+        ``panel`` columns of that block), so only diagonal blocks of at most ``leaf`` columns go through the substitution."""
+        _require_cuda(Bt)
+        if Bt.shape[2] != self.n_pad or Bt.shape[1] % TILE or Bt.stride(2) != 1:
+            raise ValueError("solve_many_rows_t_ needs a padded [B, rows_pad, n_pad] buffer")
+        self._solve_t_block(Bt, 0, self.n_pad, leaf, panel)
+        return Bt
+
+    def _solve_t_block(self, Bt, a, b, leaf, panel):
+        Lp = self.L_padded()
+        if b - a <= leaf:
+            L, X = Lp[:, a:b, a:b], Bt[:, :, a:b]
+            rc = _fn("gpk_trsm_right_t", self.dtype)(
+                _ptr(L), L.stride(1), L.stride(0), b - a, _ptr(X), X.stride(1), X.stride(0), Bt.shape[1], self.batch,
+                _stream(),
+            )
+            check(rc, "gpk_trsm_right_t")
+            return
+        m = a + round_up((b - a) // 2)
+        self._solve_t_block(Bt, m, b, leaf, panel)  # X2 L22 = B2
+        for p0 in range(a, m, panel):  # B1 -= X2 L21, `panel` columns of L21 at a time
+            p1 = min(m, p0 + panel)
+            L21t = transpose(Lp[:, m:b, p0:p1], b - m, p1 - p0)
+            gemm_nt(Bt[:, :, m:b], L21t, Bt[:, :, p0:p1], alpha=-1.0, beta=1.0)
+        self._solve_t_block(Bt, a, m, leaf, panel)  # X1 L11 = B1
 
     def half_solve(self, bt):
         """``bt [B, m, n]`` (rows = right-hand sides) -> ``(L^-1 b)^T [B, m, n]``."""

@@ -340,6 +340,13 @@ class Normal(RandomVector):
             E[:, :num, :n] = eps.transpose(1, 2)
             St = ops.gemm_nt(E, ch.L_lower_())
             s = St[:, :num, :n].transpose(1, 2).reshape(bs + (n, num))
+            from .kernels import _grad_tensors
+
+            ts = _grad_tensors(var)
+            if ts:  # L eps comes from the raw-pointer factorisation: a gradient through it would be silently wrong
+                from .autograd import no_gradient
+
+                s = no_gradient("sampling", s, ts)
         if not self.mean_is_zero:
             s = s + self._mean_dev()
         s = self._out(s)

@@ -76,6 +76,39 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase) {
       "r"(phase)
       : "memory");  // the data the barrier guards must not be read before the wait
 }
+// ---- thread-block clusters: rank, cluster-wide barrier, remote mbarrier arrive, multicast TMA (SASS: UTMALDG.MULTICAST)
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster; orders the shared-memory writes before it (mbarrier inits included) for all
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\nbarrier.cluster.wait.acquire;\n" ::: "memory");
+}
+// arrive on the mbarrier at `bar`'s shared-memory offset in CTA `rank` of the cluster (this CTA's own rank included).
+// Default (CTA-scope release) semantics, as a consumer's release of a TMA pipeline stage needs: a cluster-scope release
+// would put a MEMBAR.GPU, which waits for the thread's outstanding global reductions, in front of every arrive
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+  asm volatile(
+      "{\n"
+      ".reg .b32 remote;\n"
+      "mapa.shared::cluster.u32 remote, %0, %1;\n"
+      "mbarrier.arrive.shared::cluster.b64 _, [remote];\n"
+      "}\n" ::"r"(smem_u32(bar)),
+      "r"(rank)
+      : "memory");
+}
+// 3-D TMA box (tensor map `map`, a __grid_constant__ CUtensorMap) into `dst`'s offset in every CTA of `cta_mask`; each
+// destination CTA's mbarrier at `bar`'s offset receives the box's bytes
+__device__ __forceinline__ void tma_load_3d_multicast(void* dst, const void* map, int c0, int c1, int c2, uint64_t* bar,
+                                                      uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%2, %3, "
+      "%4}], [%5], %6;\n" ::"r"(smem_u32(dst)),
+      "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar)), "h"(cta_mask)
+      : "memory");
+}
 __device__ __forceinline__ void bulk_copy_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
   asm volatile(
       "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(

@@ -7,12 +7,16 @@
 // (they are below the slicing error), leaving S(S+1)/2 int8 GEMMs -- 21 for S = 6 (error ~2^-40 of |a||b|, zero-mean), 28
 // for S = 7 (~2^-47).
 //
-// 128 x 64 output tiles, a few consecutive tiles per CTA, enumerated in bands of tile rows, column-major inside a band (tiles
-// in flight share the band's A slices in L2; oz_tile).  Products with the same s + t share an accumulator, so a tile needs
-// S int32 accumulators per element: 128 x 64 x S does not fit the registers of two warpgroups, so every tile is computed
-// as two halves of 128 x 32 (S x 16 accumulator registers per thread, 128 for S = 8).
-//   warpgroup 0   TMA producer (one thread): per 64-byte k-block ONE box {64 B, 128 rows, S slices} of A and one
-//                 {64 B, 32 rows, S} of B (cp.async.bulk.tensor.3d, SWIZZLE_64B, mbarrier complete_tx) into a ring
+// 128 x 64 output tiles, a few consecutive tiles per cluster, enumerated in bands of tile rows, column-major inside a band
+// (tiles in flight share the band's A slices in L2; oz_tile).  Products with the same s + t share an accumulator, so a tile
+// needs S int32 accumulators per element: 128 x 64 x S does not fit the registers of two warpgroups, so every tile is
+// computed as two halves of 128 x 32 (S x 16 accumulator registers per thread, 128 for S = 8), side by side by the two
+// CTAs of a cluster: CTA rank r computes columns 32 r .. 32 r + 31 of every tile of its cluster.  Both need all 128 A rows,
+// so each loads one 64-row half of A and multicasts it into both: a tile reads its A slices from L2 once, not twice.
+//   warpgroup 0   TMA producer (one thread): per 64-byte k-block ONE box {64 B, 64 rows, S slices} of A (rows 64 r ..,
+//                 multicast to both CTAs of the cluster) and one {64 B, 32 rows, S} of B (this CTA's columns)
+//                 (cp.async.bulk.tensor.3d, SWIZZLE_64B, mbarrier complete_tx) into a ring.  A stage is laid out
+//                 [A row half][S][64 rows][64 B], then B; it is refilled once the consumers of BOTH CTAs released it
 //   warpgroups 1-2  consumers, rows 0-63 / 64-127 of the tile: per K = 32 step, slice s of A against slices 0..S-1-s of B,
 //                 grouped by PAIRS of diagonals {0,1}, {2,3}, ... (B slices adjacent in shared memory, accumulators
 //                 adjacent in the register fragment): for each group {lo, lo+1} with lo > s - 1 one wgmma with N = 64 (32
@@ -57,12 +61,13 @@ struct OzCfg {
   static constexpr int EXTRA = PAD ? 0 : S / 2;
   static constexpr int ACC = 16 * (S + EXTRA);  // int32 accumulator registers per thread
   static constexpr int RA = (192 - ACC) / 8 < S ? (192 - ACC) / 8 : S;
-  static constexpr int A_SLICE = OZ_BM * OZ_BK;  // 8 KB
+  static constexpr int A_SLICE = 64 * OZ_BK;     // 4 KB: one 64-row half of an A slice
+  static constexpr int A_HALF = S * A_SLICE;     // a row half, all slices: one multicast box, one consumer warpgroup's rows
   static constexpr int B_SLICE = OZ_HN * OZ_BK;  // 2 KB
-  static constexpr int A_BYTES = S * A_SLICE;
+  static constexpr int A_BYTES = 2 * A_HALF;
   static constexpr int Z_BYTES = PAD ? B_SLICE : 0;
   static constexpr int B_BYTES = S * B_SLICE;
-  static constexpr int TX_BYTES = A_BYTES + B_BYTES;  // what the TMA writes per stage
+  static constexpr int TX_BYTES = A_BYTES + B_BYTES;  // what the TMA writes per stage: both A halves (own + peer) and B
   static constexpr int STAGE_BYTES = A_BYTES + Z_BYTES + B_BYTES;
   static constexpr int SMEM_MAX = 226 * 1024;  // 227 KB per CTA minus the static barriers / alignment slack
   static constexpr int STAGES = (SMEM_MAX - 1024) / STAGE_BYTES > 4 ? 4 : (SMEM_MAX - 1024) / STAGE_BYTES;
@@ -96,8 +101,19 @@ __device__ __forceinline__ void oz_mbar_wait(uint64_t* bar, uint32_t parity) {
       "r"(parity)
       : "memory");
 }
-__device__ __forceinline__ void oz_mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(bar)) : "memory");
+// the producer's wait for a free stage: the releases come from the consumers of both CTAs (mbar_arrive_cluster)
+__device__ __forceinline__ void oz_mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
+  asm volatile(
+      "{\n"
+      ".reg .pred P1;\n"
+      "OZC_LOOP:\n"
+      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 P1, [%0], %1;\n"
+      "@P1 bra OZC_DONE;\n"
+      "bra OZC_LOOP;\n"
+      "OZC_DONE:\n"
+      "}\n" ::"r"(smem_u32(bar)),
+      "r"(parity)
+      : "memory");
 }
 __device__ __forceinline__ void oz_tma_load_3d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
   asm volatile(
@@ -183,16 +199,18 @@ __host__ __device__ __forceinline__ void oz_tile(const OzParams& p, int t, int& 
   tn = p.tiles_n - 1;
 }
 
-// One CTA works through `tiles_per_cta` consecutive tiles, each as two 128 x 32 halves: the TMA producer runs ahead through
-// the ring into the next half / tile while the consumers finish the current one.  CTAs stay short-lived (a few tiles) on
-// purpose: the Cholesky's look-ahead stream needs SMs to come free every few tens of us.
+// Launched as clusters of 2 CTAs (oz_launch_gemm).  A cluster works through `tiles_per_cta` consecutive tiles; CTA rank r
+// computes the 128 x 32 half r of each.  The TMA producer runs ahead through the ring into the next tile while the
+// consumers finish the current one.  Both CTAs walk the same tiles and k-blocks, so their rings stay in step.  Clusters
+// stay short-lived (a few tiles) on purpose: the Cholesky's look-ahead stream needs SMs to come free every few tens of us.
 template <int S>
 __global__ void __launch_bounds__(OZ_THREADS, 1)
 oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const OzParams p) {
   using Cfg = OzCfg<S>;
   constexpr int STAGES = Cfg::STAGES;
   const int wg = threadIdx.x >> 7;
-  const int t_begin = blockIdx.x * p.tiles_per_cta;
+  const uint32_t rank = cluster_ctarank();  // A row half this CTA loads for both, column half of every tile it computes
+  const int t_begin = (blockIdx.x >> 1) * p.tiles_per_cta;
   const int t_end = min(t_begin + p.tiles_per_cta, p.total_tiles);
 
   extern __shared__ uint8_t oz_smem_raw[];
@@ -201,8 +219,8 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 256);  // every consumer thread, after its warpgroup's MMAs on the stage completed
+      mbar_init(&full_bar[s], 1);  // this CTA's producer (expect_tx of both A halves and B)
+      mbar_init(&empty_bar[s], 2 * 8);  // lane 0 of each of the 8 consumer warps of BOTH CTAs, after its MMAs on the stage
     }
     fence_mbar_init();
   }
@@ -213,7 +231,7 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     }
     asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
   }
-  __syncthreads();
+  cluster_sync();  // no multicast or remote arrive may reach the peer's barriers before it initialised them
   const int KB = p.KB;
 
   if (wg == 0) {
@@ -223,36 +241,38 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
       for (int t = t_begin; t < t_end; ++t) {
         int tm, tn;
         oz_tile(p, t, tm, tn);
-        for (int h = 0; h < 2; ++h) {
-          for (int kb = 0; kb < KB; ++kb, ++g) {
-            const int s = g % STAGES, it = g / STAGES;
-            if (it > 0) oz_mbar_wait(&empty_bar[s], (it - 1) & 1);
-            uint8_t* st = smem + s * Cfg::STAGE_BYTES;
-            mbar_arrive_expect_tx(&full_bar[s], Cfg::TX_BYTES);
-            oz_tma_load_3d(st, &mapA, kb * OZ_BK, p.a_row0 + tm * OZ_BM, 0, &full_bar[s]);
-            oz_tma_load_3d(st + Cfg::A_BYTES + Cfg::Z_BYTES, &mapB, kb * OZ_BK, p.b_row0 + tn * OZ_BN + h * OZ_HN, 0, &full_bar[s]);
-          }
+        for (int kb = 0; kb < KB; ++kb, ++g) {
+          const int s = g % STAGES, it = g / STAGES;
+          if (it > 0) oz_mbar_wait_cluster(&empty_bar[s], (it - 1) & 1);  // both CTAs done with the stage's last use
+          uint8_t* st = smem + s * Cfg::STAGE_BYTES;
+          mbar_arrive_expect_tx(&full_bar[s], Cfg::TX_BYTES);
+          tma_load_3d_multicast(st + rank * Cfg::A_HALF, &mapA, kb * OZ_BK, p.a_row0 + tm * OZ_BM + 64 * rank, 0,
+                                &full_bar[s], 0x3);
+          oz_tma_load_3d(st + Cfg::A_BYTES + Cfg::Z_BYTES, &mapB, kb * OZ_BK, p.b_row0 + tn * OZ_BN + rank * OZ_HN, 0,
+                         &full_bar[s]);
         }
       }
+      // before this CTA may exit: the last use of every stage released by the consumers of BOTH CTAs, i.e. every remote
+      // arrive on our barriers has landed (every multicast into our stages has, since our consumers waited for them).
+      // Cheaper than a cluster barrier with release semantics, whose MEMBAR.GPU waits for the epilogue's reductions
+      for (int u = g > STAGES ? g - STAGES : 0; u < g; ++u) oz_mbar_wait_cluster(&empty_bar[u % STAGES], (u / STAGES) & 1);
     }
-    return;
-  }
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::);
-  const int tid = threadIdx.x - 128 * wg, wrow = 64 * (wg - 1);  // thread in the warpgroup, first tile row it owns
-  const int r_lo = 16 * (tid >> 5) + ((tid & 31) >> 2), c_lo = 2 * (tid & 3);
-  // 2^-(12 + 7 (S-1)): weight of the last kept diagonal; Horner runs from diagonal 0 (largest weight) down
-  const double w_last = __hiloint2double((1023 - (12 + 7 * (S - 1))) << 20, 0);
-  // ldmatrix.x4 source of this lane inside an A slice, for the two K = 32 halves of the 64-byte (SWIZZLE_64B) row: matrix
-  // lane / 8 = rows +8 (bit 0) and bytes +16 (bit 1), 16-byte chunk XOR (row / 2) % 4
-  const int lane = tid & 31, a_row = wrow + 16 * (tid >> 5) + (lane & 7) + 8 * ((lane >> 3) & 1);
-  const uint32_t a_off0 = a_row * OZ_BK + ((((lane >> 4) + 0) ^ ((lane >> 1) & 3)) << 4);
-  const uint32_t a_off1 = a_row * OZ_BK + ((((lane >> 4) + 2) ^ ((lane >> 1) & 3)) << 4);
-  uint32_t acc[Cfg::ACC];
-  int g = 0;
-  for (int t = t_begin; t < t_end; ++t) {
-    int tm, tn;
-    oz_tile(p, t, tm, tn);
-    for (int h = 0; h < 2; ++h) {
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::);
+    const int tid = threadIdx.x - 128 * wg, half = wg - 1;  // thread in the warpgroup, the A row half (64 rows) it owns
+    const int r_lo = 16 * (tid >> 5) + ((tid & 31) >> 2), c_lo = 2 * (tid & 3);
+    // 2^-(12 + 7 (S-1)): weight of the last kept diagonal; Horner runs from diagonal 0 (largest weight) down
+    const double w_last = __hiloint2double((1023 - (12 + 7 * (S - 1))) << 20, 0);
+    // ldmatrix.x4 source of this lane inside its row half of an A slice, for the two K = 32 halves of the 64-byte
+    // (SWIZZLE_64B) row: matrix lane / 8 = rows +8 (bit 0) and bytes +16 (bit 1), 16-byte chunk XOR (row / 2) % 4
+    const int lane = tid & 31, a_row = 16 * (tid >> 5) + (lane & 7) + 8 * ((lane >> 3) & 1);
+    const uint32_t a_off0 = half * Cfg::A_HALF + a_row * OZ_BK + ((((lane >> 4) + 0) ^ ((lane >> 1) & 3)) << 4);
+    const uint32_t a_off1 = half * Cfg::A_HALF + a_row * OZ_BK + ((((lane >> 4) + 2) ^ ((lane >> 1) & 3)) << 4);
+    uint32_t acc[Cfg::ACC];
+    int g = 0;
+    for (int t = t_begin; t < t_end; ++t) {
+      int tm, tn;
+      oz_tile(p, t, tm, tn);
       // ---- main loop: all wgmmas of a k-block in flight at once, A fragments in registers ----
       for (int kb = 0; kb < KB; ++kb, ++g) {
         const int s = g % STAGES, it = g / STAGES;
@@ -267,10 +287,13 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
         wgmma_fence();
 #pragma unroll
         for (int ks = 0; ks < 2; ++ks)  // wgmma K = 32 int8 = 32 bytes inside the 64-byte swizzle row
-          oz_mma_step<S, 0>(acc, a[ks], st + wrow * OZ_BK + ks * 32, b0 + ks * 32, (kb > 0 || ks > 0) ? 1u : 0u);
+          oz_mma_step<S, 0>(acc, a[ks], st + half * Cfg::A_HALF + ks * 32, b0 + ks * 32, (kb > 0 || ks > 0) ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<0>();  // (the A registers are rewritten by the next k-block; the other consumer keeps the tensor cores busy)
-        oz_mbar_arrive(&empty_bar[s]);
+        if (lane == 0) {  // the stage is free for this warp in both CTAs (the peer multicasts its A half into ours)
+          mbar_arrive_cluster(&empty_bar[s], 0);
+          mbar_arrive_cluster(&empty_bar[s], 1);
+        }
       }
       // ---- epilogue: Horner-combine the diagonals in fp64, scale, add into C ----
       if constexpr (Cfg::EXTRA > 0) {  // fold the extra accumulators into their diagonals (exact int32 sums)
@@ -279,8 +302,8 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
 #pragma unroll
           for (int i = 0; i < 16; ++i) acc[16 * d + i] += acc[16 * (S + d / 2) + i];
       }
-      const int64_t row0 = (int64_t)tm * OZ_BM + wrow + r_lo;
-      const int64_t col0 = (int64_t)tn * OZ_BN + h * OZ_HN + c_lo;
+      const int64_t row0 = (int64_t)tm * OZ_BM + 64 * half + r_lo;
+      const int64_t col0 = (int64_t)tn * OZ_BN + rank * OZ_HN + c_lo;
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
         const int64_t row = row0 + 8 * ((i >> 1) & 1), col = col0 + 8 * (i >> 2) + (i & 1);
@@ -390,7 +413,7 @@ int oz_launch_gemm(int64_t M, int64_t N, int64_t K, double alpha, const int8_t* 
                    const double* scB, int64_t rowB, double beta, double* C, int64_t ldc, int32_t lower,
                    cudaStream_t stream) {
   CUtensorMap mA, mB;
-  if (!oz_make_map(&mA, planesA, K, capA, strideA, S, OZ_BM) || !oz_make_map(&mB, planesB, K, capB, strideB, S, OZ_HN))
+  if (!oz_make_map(&mA, planesA, K, capA, strideA, S, OZ_BM / 2) || !oz_make_map(&mB, planesB, K, capB, strideB, S, OZ_HN))
     return GPK_ERR_UNSUPPORTED;
   if (const int rc = opt_in_smem<oz_gemm_kernel<S>>(OzCfg<S>::SMEM_BYTES)) return rc;
   if (beta != 0.0 && beta != 1.0) {  // the kernel adds into C (or overwrites it): apply any other beta first
@@ -401,10 +424,11 @@ int oz_launch_gemm(int64_t M, int64_t N, int64_t K, double alpha, const int8_t* 
   const int32_t tiles_m = (int32_t)(M / OZ_BM), tiles_n = (int32_t)(N / OZ_BN);
   const int32_t tri_rows = lower ? (tiles_m < tiles_n / 2 ? tiles_m : tiles_n / 2) : 0;
   const int32_t total = lower ? tri_rows * (tri_rows + 1) + (tiles_m - tri_rows) * tiles_n : tiles_m * tiles_n;
-  // tiles per CTA: >= 2 waves of CTAs over the H100's 132 SMs before CTAs grow, and CTAs stay short-lived (look-ahead
-  // streams need SMs every few tens of us)
+  // tiles per cluster: >= 2 waves of CTAs (132 clusters of 2) over the H100's 132 SMs before clusters grow, and CTAs stay
+  // short-lived (look-ahead streams need SMs every few tens of us): at most 2 tiles at K > 512, 4 below.  At n = 16384
+  // (400 W H100) the log-pdf step was 1.7 % slower with caps of 4 / 8, and 8 / 16 was another 3.3 % slower than 4 / 8
   const int32_t tpc_cap = K > 512 ? 2 : 4;
-  int32_t tpc = total / 264;
+  int32_t tpc = total / 132;
   tpc = tpc < 1 ? 1 : (tpc > tpc_cap ? tpc_cap : tpc);
   // band height of the tile order: as many tile rows as keep the band's A slices (128 K S bytes per tile row) within ~12 MB
   // of the H100's 50 MB L2, at most 16 (K = 1024, S = 7: 13 rows = 11.4 MB; the K = 8192 products of the triangular solves: 1-2 rows)
@@ -414,8 +438,21 @@ int oz_launch_gemm(int64_t M, int64_t N, int64_t K, double alpha, const int8_t* 
              tiles_m, tiles_n, total, tpc, tri_rows, beta != 0.0 ? 1 : 0, band};
   // profile: algorithmic (fp64-equivalent) flops of the tiles computed; the int8 work is S (S + 1) / 2 times that
   if (prof_enabled()) prof_begin(stream, (double)total * 2.0 * OZ_BM * OZ_BN * (double)K, 1);
-  oz_gemm_kernel<S><<<(unsigned)((total + tpc - 1) / tpc), OZ_THREADS, OzCfg<S>::SMEM_BYTES, stream>>>(mA, mB, p);
+  cudaLaunchAttribute cluster;
+  cluster.id = cudaLaunchAttributeClusterDimension;
+  cluster.val.clusterDim.x = 2;  // the kernel's CTA pair: one column half of each tile each, A multicast to both
+  cluster.val.clusterDim.y = 1;
+  cluster.val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(2 * (unsigned)((total + tpc - 1) / tpc));
+  cfg.blockDim = dim3(OZ_THREADS);
+  cfg.dynamicSmemBytes = OzCfg<S>::SMEM_BYTES;
+  cfg.stream = stream;
+  cfg.attrs = &cluster;
+  cfg.numAttrs = 1;
+  const cudaError_t le = cudaLaunchKernelEx(&cfg, oz_gemm_kernel<S>, mA, mB, p);
   if (prof_enabled()) prof_end(stream);
+  if (le != cudaSuccess) return -1000 - (int)le;
   GPK_COUNT_LAUNCH();
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : -1000 - (int)e;

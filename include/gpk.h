@@ -186,7 +186,10 @@ int gpk_set_f64_emulation(int32_t slices, void* scratch, int64_t scratch_bytes);
 int64_t gpk_f64_emulation_scratch_bytes(int64_t M, int64_t N, int64_t K, int32_t slices);
 
 /* The emulated GEMM on its own: C = beta C + alpha A B^T (M % 128 == 0, N % 64 == 0, K % 128 == 0, K <= 65536).
- * `ws`: 1024-byte aligned, >= round_up(gpk_oz_ws_bytes(M, K, slices), 1024) + gpk_oz_ws_bytes(N, K, slices) bytes. */
+ * `ws`: 1024-byte aligned, >= round_up(gpk_oz_ws_bytes(M, K, slices), 1024) + gpk_oz_ws_bytes(N, K, slices) bytes.
+ * Rows of every finite magnitude are scaled exactly (subnormal to near overflow); a row of A (B) holding a NaN or an
+ * infinity makes its row (column) of alpha A B^T NaN, where fp64 gives NaN or +-inf.  Lower mode and beta as in
+ * gpk_gemm_nt_f64: only the tiles that touch the lower triangle are read or written, for every beta. */
 int64_t gpk_oz_ws_bytes(int64_t rows, int64_t K, int32_t slices);
 int gpk_gemm_nt_f64_oz(int64_t M, int64_t N, int64_t K, double alpha, const double* A, int64_t lda, const double* B,
                        int64_t ldb, double beta, double* C, int64_t ldc, int32_t lower, int32_t slices, void* ws,

@@ -30,6 +30,9 @@
 //                 shared memory.  Then the epilogue: Horner-combine the S diagonals in fp64 (exact int32 -> double
 //                 through the 2^52 trick), scale by 2^(e_row + e_col) and add into C (red.global.add.f64: the
 //                 read-modify-write happens in L2, as one correctly rounded addition per element)
+// Rows of every finite magnitude (subnormal to near overflow) are scaled exactly, and the exponents are summed as integers
+// before the scale is applied, so products of very small rows with very large ones keep the full accuracy.  A row with a
+// NaN or an infinity makes its whole row (column) of the product NaN -- where fp64 gives NaN or +-inf.
 // The slicing kernel (oz_slice_kernel) is O(rows*K) and runs once per panel; in the Cholesky its output is shared by
 // every tile of the trailing update.  Every inexact step is ONE correctly rounded fp64 operation, so the result equals a
 // NumPy integer model of the algorithm bit for bit (tests/_oz_model.py, tests/test_emulation.py).
@@ -75,11 +78,25 @@ struct OzCfg {
   static_assert(STAGES >= 2, "ring");
 };
 
+// Row exponent of a row holding a NaN or an infinity: every element of the product that the row touches becomes NaN
+constexpr int32_t OZ_E_NONFINITE = 1 << 20;
+
+// 2^e for e in [-1022, 1023] (a normal double)
+__device__ __forceinline__ double oz_pow2(int e) { return __hiloint2double((1023 + e) << 20, 0); }
+
+// x 2^E for E outside the normal range: two normal powers of two, the larger one first (x 2^-1022 stays exact for |x| >= 1,
+// so only the last product rounds); NaN for the exponent of a non-finite row
+__device__ __forceinline__ double oz_scale_wide(double x, int E) {
+  if (E > OZ_E_NONFINITE / 2) return __longlong_as_double(0x7ff8000000000000ll);
+  const int e1 = E < 0 ? -1022 : 1023;
+  return x * oz_pow2(e1) * oz_pow2(max(E - e1, -1022));
+}
+
 struct OzParams {
   double alpha;
   double* C;
-  const double* sc_a;  // 2^e per A row (already offset to the first row of the problem)
-  const double* sc_b;
+  const int32_t* ex_a;  // row exponent e per A row (already offset to the first row of the problem)
+  const int32_t* ex_b;
   int64_t ldc;
   int32_t a_row0, b_row0;  // first plane row of A / B
   int32_t KB, lower, tiles_m, tiles_n;
@@ -261,8 +278,6 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::);
     const int tid = threadIdx.x - 128 * wg, half = wg - 1;  // thread in the warpgroup, the A row half (64 rows) it owns
     const int r_lo = 16 * (tid >> 5) + ((tid & 31) >> 2), c_lo = 2 * (tid & 3);
-    // 2^-(12 + 7 (S-1)): weight of the last kept diagonal; Horner runs from diagonal 0 (largest weight) down
-    const double w_last = __hiloint2double((1023 - (12 + 7 * (S - 1))) << 20, 0);
     // ldmatrix.x4 source of this lane inside its row half of an A slice, for the two K = 32 halves of the 64-byte
     // (SWIZZLE_64B) row: matrix lane / 8 = rows +8 (bit 0) and bytes +16 (bit 1), 16-byte chunk XOR (row / 2) % 4
     const int lane = tid & 31, a_row = 16 * (tid >> 5) + (lane & 7) + 8 * ((lane >> 3) & 1);
@@ -304,14 +319,54 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
       }
       const int64_t row0 = (int64_t)tm * OZ_BM + 64 * half + r_lo;
       const int64_t col0 = (int64_t)tn * OZ_BN + rank * OZ_HN + c_lo;
+      // Scaling: out = v alpha 2^E, E = e_row + e_col - W (W: the weight of the last kept diagonal; Horner ran from
+      // diagonal 0 down), rounded once.  This thread's 2 rows and 8 columns give factors ra = alpha 2^(e_row - W) and
+      // cb = 2^e_col.  When all of them and all their products are normal doubles (the usual case), ra cb = alpha 2^E
+      // exactly and out = v (ra cb) is that one rounding.  Otherwise (rows far from 1, non-finite rows) E is summed as
+      // an integer per element and applied last to v alpha, in two power-of-two factors when it lies outside the normal
+      // range: one rounding for every normal result, and nothing goes subnormal before the result does
+      constexpr int W = 12 + 7 * (S - 1);
+      double ra[2], cb[8];
+      bool fast = true;
+      double ra_min = 1.0 / 0.0, ra_max = 0.0;
+      int eb_min = 1023, eb_max = -1022;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int e = __ldg(p.ex_a + row0 + 8 * h) - W;
+        fast = fast && (unsigned)(e + 1022) <= 2045u;
+        ra[h] = p.alpha * oz_pow2(min(max(e, -1022), 1023));
+        ra_min = fmin(ra_min, fabs(ra[h]));
+        ra_max = fmax(ra_max, fabs(ra[h]));
+      }
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const int e = __ldg(p.ex_b + col0 + 8 * (q >> 1) + (q & 1));
+        fast = fast && (unsigned)(e + 1022) <= 2045u;
+        eb_min = min(eb_min, e);
+        eb_max = max(eb_max, e);
+        cb[q] = oz_pow2(min(max(e, -1022), 1023));
+      }
+      constexpr double DBL_MIN_NORMAL = 2.2250738585072014e-308;
+      fast = fast && ra_min >= DBL_MIN_NORMAL && ra_max <= 1.7976931348623157e308 &&
+             ra_min * oz_pow2(max(eb_min, -1022)) >= DBL_MIN_NORMAL &&
+             ra_max * oz_pow2(min(eb_max, 1023)) <= 1.7976931348623157e308;
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
         const int64_t row = row0 + 8 * ((i >> 1) & 1), col = col0 + 8 * (i >> 2) + (i & 1);
         double v = oz_i2d(acc[i]);
 #pragma unroll
         for (int d = 1; d < S; ++d) v = fma(v, 128.0, oz_i2d(acc[16 * d + i]));
-        const double rs = p.alpha * w_last * __ldg(p.sc_a + row);
-        const double out = v * (rs * __ldg(p.sc_b + col));
+        double out;
+        if (fast) {
+          out = v * (ra[(i >> 1) & 1] * cb[2 * (i >> 2) + (i & 1)]);
+        } else {
+          const int E = __ldg(p.ex_a + row) + __ldg(p.ex_b + col) - W;
+          out = v * p.alpha;
+          if ((unsigned)(E + 1022) <= 2045u)
+            out *= oz_pow2(E);
+          else
+            out = oz_scale_wide(out, E);
+        }
         double* c = p.C + row * p.ldc + col;
         if (p.accumulate)
           atomicAdd(c, out);
@@ -322,33 +377,45 @@ oz_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   }
 }
 
-// ---- slicing: one warp per row.  planes[s][row][k] (int8), sc[row] = 2^e -----------------------------------------------
+// ---- slicing: one warp per row.  planes[s][row][k] (int8), ex[row] = e -------------------------------------------------
+// e = ilogb(row max) + 1 over the whole finite range (subnormal rows included: e in [-1073, 1024]), 0 for an all-zero row.
+// A row holding a NaN or an infinity gets e = OZ_E_NONFINITE and zero slices: its row (column) of the product is NaN, as
+// it is in fp64 -- and a factorisation then reports the first pivot the non-finite value reaches, as the native path does.
 template <int S>
 __global__ void __launch_bounds__(256)
 oz_slice_kernel(const double* __restrict__ P, int64_t ldp, int64_t rows, int32_t K, int8_t* __restrict__ planes,
-                int64_t plane_stride, double* __restrict__ sc) {
+                int64_t plane_stride, int32_t* __restrict__ ex) {
   const int64_t row = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
   const double* src = P + row * ldp;
   double m = 0.0;
+  bool finite = true;
   for (int k = lane * 4; k < K; k += 128) {
     const double2 a = *reinterpret_cast<const double2*>(src + k), b = *reinterpret_cast<const double2*>(src + k + 2);
     m = fmax(fmax(fabs(a.x), fabs(a.y)), fmax(m, fmax(fabs(b.x), fabs(b.y))));
+    finite = finite && isfinite(a.x) && isfinite(a.y) && isfinite(b.x) && isfinite(b.y);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+  finite = __all_sync(0xffffffffu, finite);
+  // r = x 2^-e, as two exact power-of-two scalings (2^-e itself is not a double for e < -1022 or e > 1023)
   int e = 0;
-  if (m > 0.0 && m < 1e300) {  // (inf / nan rows: the factorisation reports them through `info` anyway)
+  double inv1 = finite ? 1.0 : 0.0, inv2 = 1.0;
+  if (!finite) {
+    e = OZ_E_NONFINITE;
+  } else if (m > 0.0) {
     e = ilogb(m) + 1;
-    e = max(-1000, min(1000, e));
+    const int s1 = min(max(-e, -1022), 1023);
+    inv1 = oz_pow2(s1);
+    inv2 = oz_pow2(-e - s1);
   }
-  const double inv = __hiloint2double((1023 - e) << 20, 0);  // 2^-e
-  if (lane == 0) sc[row] = __hiloint2double((1023 + e) << 20, 0);
+  if (lane == 0) ex[row] = e;
   int8_t* dst = planes + row * K;
   for (int k = lane * 4; k < K; k += 128) {
     const double2 a = *reinterpret_cast<const double2*>(src + k), b = *reinterpret_cast<const double2*>(src + k + 2);
-    double r[4] = {a.x * inv, a.y * inv, b.x * inv, b.y * inv};
+    double r[4] = {a.x * inv1 * inv2, a.y * inv1 * inv2, b.x * inv1 * inv2, b.y * inv1 * inv2};
+    if (!finite) r[0] = r[1] = r[2] = r[3] = 0.0;
     double pw = 64.0, ipw = 1.0 / 64.0;
 #pragma unroll
     for (int s = 0; s < S; ++s) {
@@ -393,32 +460,34 @@ bool oz_make_map(CUtensorMap* m, const int8_t* planes, int64_t K, int64_t rows_c
 }
 
 template <int S>
-int oz_launch_slice(const double* P, int64_t ldp, int64_t rows, int64_t K, int8_t* planes, int64_t plane_stride, double* sc,
+int oz_launch_slice(const double* P, int64_t ldp, int64_t rows, int64_t K, int8_t* planes, int64_t plane_stride, int32_t* ex,
                     cudaStream_t stream) {
   if (rows == 0) return 0;
-  oz_slice_kernel<S><<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(P, ldp, rows, (int32_t)K, planes, plane_stride, sc);
+  oz_slice_kernel<S><<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(P, ldp, rows, (int32_t)K, planes, plane_stride, ex);
   GPK_COUNT_LAUNCH();
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : -1000 - (int)e;
 }
 
-__global__ void oz_scale_kernel(double* C, int64_t ldc, int64_t M, int64_t N, double beta) {
-  const int64_t i = (int64_t)blockIdx.y, j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < M && j < N) C[i * ldc + j] *= beta;
+// C *= beta on the elements the GEMM kernel writes: all of C, or in lower mode the tiles that touch the lower triangle
+// (row i: columns below 128 (i / 128 + 1)).  One block per row.
+__global__ void oz_scale_kernel(double* C, int64_t ldc, int64_t N, double beta, int32_t lower) {
+  const int64_t i = (int64_t)blockIdx.x;
+  const int64_t n = lower ? min(N, (i / OZ_BM + 1) * OZ_BM) : N;
+  for (int64_t j = threadIdx.x; j < n; j += blockDim.x) C[i * ldc + j] *= beta;
 }
 
 template <int S>
 int oz_launch_gemm(int64_t M, int64_t N, int64_t K, double alpha, const int8_t* planesA, int64_t capA, int64_t strideA,
-                   const double* scA, int64_t rowA, const int8_t* planesB, int64_t capB, int64_t strideB,
-                   const double* scB, int64_t rowB, double beta, double* C, int64_t ldc, int32_t lower,
+                   const int32_t* exA, int64_t rowA, const int8_t* planesB, int64_t capB, int64_t strideB,
+                   const int32_t* exB, int64_t rowB, double beta, double* C, int64_t ldc, int32_t lower,
                    cudaStream_t stream) {
   CUtensorMap mA, mB;
   if (!oz_make_map(&mA, planesA, K, capA, strideA, S, OZ_BM / 2) || !oz_make_map(&mB, planesB, K, capB, strideB, S, OZ_HN))
     return GPK_ERR_UNSUPPORTED;
   if (const int rc = opt_in_smem<oz_gemm_kernel<S>>(OzCfg<S>::SMEM_BYTES)) return rc;
   if (beta != 0.0 && beta != 1.0) {  // the kernel adds into C (or overwrites it): apply any other beta first
-    if (M > 65535) return GPK_ERR_UNSUPPORTED;
-    oz_scale_kernel<<<dim3((unsigned)((N + 255) / 256), (unsigned)M), 256, 0, stream>>>(C, ldc, M, N, beta);
+    oz_scale_kernel<<<(unsigned)M, 256, 0, stream>>>(C, ldc, N, beta, lower);
     GPK_COUNT_LAUNCH();
   }
   const int32_t tiles_m = (int32_t)(M / OZ_BM), tiles_n = (int32_t)(N / OZ_BN);
@@ -434,7 +503,7 @@ int oz_launch_gemm(int64_t M, int64_t N, int64_t K, double alpha, const int8_t* 
   // of the H100's 50 MB L2, at most 16 (K = 1024, S = 7: 13 rows = 11.4 MB; the K = 8192 products of the triangular solves: 1-2 rows)
   int32_t band = (int32_t)((12ll << 20) / (128ll * K * S));
   band = band < 1 ? 1 : (band > 16 ? 16 : band);
-  OzParams p{alpha, C, scA + rowA, scB + rowB, ldc, (int32_t)rowA, (int32_t)rowB, (int32_t)(K / OZ_BK), lower,
+  OzParams p{alpha, C, exA + rowA, exB + rowB, ldc, (int32_t)rowA, (int32_t)rowB, (int32_t)(K / OZ_BK), lower,
              tiles_m, tiles_n, total, tpc, tri_rows, beta != 0.0 ? 1 : 0, band};
   // profile: algorithmic (fp64-equivalent) flops of the tiles computed; the int8 work is S (S + 1) / 2 times that
   if (prof_enabled()) prof_begin(stream, (double)total * 2.0 * OZ_BM * OZ_BN * (double)K, 1);
@@ -461,19 +530,20 @@ int oz_launch_gemm(int64_t M, int64_t N, int64_t K, double alpha, const int8_t* 
 }  // namespace
 
 // ---- entry points used by potrf.cu and the C-ABI ----------------------------------------------------------------------
-// workspace for `rows` rows of K columns: S int8 planes [S][rows][K] followed by `rows` doubles (the row scales)
+// workspace for `rows` rows of K columns: S int8 planes [S][rows][K] followed by the `rows` row exponents (int32, in 8
+// bytes per row)
 int64_t oz_ws_bytes(int64_t rows, int64_t K, int32_t S) { return (int64_t)S * rows * K + rows * 8 + 256; }
 
-static inline double* oz_scales(void* ws, int64_t rows, int64_t K, int32_t S) {
+static inline int32_t* oz_exponents(void* ws, int64_t rows, int64_t K, int32_t S) {
   const uintptr_t p = reinterpret_cast<uintptr_t>(ws) + (uintptr_t)((int64_t)S * rows * K);
-  return reinterpret_cast<double*>((p + 255) & ~uintptr_t(255));
+  return reinterpret_cast<int32_t*>((p + 255) & ~uintptr_t(255));
 }
 
 int oz_slice_panel(const double* P, int64_t ldp, int64_t rows, int64_t K, void* ws, int64_t cap_rows, int32_t S,
                    cudaStream_t stream) {
   if (K % 128 || K > 65536 || rows > cap_rows || ldp % 2 || reinterpret_cast<uintptr_t>(P) % 16) return GPK_ERR_ARG;
   int8_t* planes = static_cast<int8_t*>(ws);
-  double* sc = oz_scales(ws, cap_rows, K, S);
+  int32_t* sc = oz_exponents(ws, cap_rows, K, S);
   switch (S) {
     case 5: return oz_launch_slice<5>(P, ldp, rows, K, planes, cap_rows * K, sc, stream);
     case 6: return oz_launch_slice<6>(P, ldp, rows, K, planes, cap_rows * K, sc, stream);
@@ -491,8 +561,8 @@ int oz_gemm_sliced(int64_t M, int64_t N, int64_t K, double alpha, const void* ws
   if (M == 0 || N == 0) return 0;
   const int8_t* pa = static_cast<const int8_t*>(wsA);
   const int8_t* pb = static_cast<const int8_t*>(wsB);
-  const double* sa = oz_scales(const_cast<void*>(wsA), capA, K, S);
-  const double* sb = oz_scales(const_cast<void*>(wsB), capB, K, S);
+  const int32_t* sa = oz_exponents(const_cast<void*>(wsA), capA, K, S);
+  const int32_t* sb = oz_exponents(const_cast<void*>(wsB), capB, K, S);
 #define OZ_CASE(SS)                                                                                                   \
   case SS:                                                                                                            \
     return oz_launch_gemm<SS>(M, N, K, alpha, pa, capA, capA * K, sa, rowA, pb, capB, capB * K, sb, rowB, beta, C, ldc, \

@@ -543,6 +543,11 @@ def gemm_nt_oz(A, Bm, C=None, *, alpha=1.0, beta=0.0, lower=False, slices=6):
     N = Bm.shape[0]
     if C is None:
         C = torch.zeros(M, N, device=A.device, dtype=A.dtype)
+    for t in (A, Bm, C):
+        if t.dim() != 2 or t.stride(1) != 1 or t.dtype != torch.float64:
+            raise ValueError("gemm_nt_oz takes fp64 matrices with a unit inner stride")
+    if Bm.shape[1] != K or C.shape != (M, N):
+        raise ValueError("gemm_nt_oz: shapes do not match")
     lib = _lib.load()
     need = ((lib.gpk_oz_ws_bytes(M, K, slices) + 1023) // 1024) * 1024 + lib.gpk_oz_ws_bytes(N, K, slices)
     ws = _aligned_bytes(need, A.device)

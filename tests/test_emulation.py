@@ -63,12 +63,14 @@ def test_gemm_oz_lower_and_zero_rows(ops):
     P = torch.randn(512, 256, device="cuda", dtype=torch.float64, generator=g)
     P[100:140] = 0.0  # all-zero rows (identity padding produces them)
     C0 = torch.randn(512, 512, device="cuda", dtype=torch.float64, generator=g)
-    C = ops.gemm_nt_oz(P, P, C0.clone(), alpha=-1.0, beta=1.0, lower=True, slices=7)
-    ref = C0 - P @ P.T
     mask = torch.ones(512, 512, device="cuda", dtype=torch.bool).tril()
-    assert ((C - ref)[mask].abs().max() / ref.abs().max()).item() < 1e-13
-    # tiles strictly above the diagonal (128 x 64 granularity) are not touched
-    assert torch.equal(C[:128, 128:], C0[:128, 128:])
+    above = torch.arange(512, device="cuda")[None, :] >= 128 * (torch.arange(512, device="cuda")[:, None] // 128 + 1)
+    for beta in (1.0, 0.5):
+        C = ops.gemm_nt_oz(P, P, C0.clone(), alpha=-1.0, beta=beta, lower=True, slices=7)
+        ref = beta * C0 - P @ P.T
+        assert ((C - ref)[mask].abs().max() / ref.abs().max()).item() < 1e-13
+        # tiles strictly above the diagonal (128 x 64 granularity) are not touched, whatever beta
+        assert torch.equal(C[above], C0[above])
 
 
 @pytest.mark.parametrize("n,k", [(2048, 1), (3000, 3), (4480, 1)])
@@ -187,10 +189,19 @@ def test_gemm_oz_bit_exact_vs_integer_model(ops, slices, alpha, beta):
     A = rng.standard_normal((M, K)) * np.exp(2 * rng.standard_normal((M, 1)))
     B = rng.standard_normal((N, K))
     C0 = rng.standard_normal((M, N))
+    # rows from subnormal to near overflow (their products with each other O(1), with the other rows anything from zero
+    # through subnormal to inf), and rows holding a NaN or an infinity
+    for r, k in enumerate((-1070, -1020, -1000, -980, 980, 1000, 1020)):
+        A[200 + r] = np.ldexp(rng.standard_normal(K), k)
+        B[100 + r] = np.ldexp(rng.standard_normal(K), min(-k, 1020))
+    A[220, 7], A[221, 300], B[120, 0] = np.nan, np.inf, -np.inf
     want = oz_model_gemm(A, B, C0, alpha, beta, slices)
     dev = lambda a: torch.as_tensor(a, device="cuda")
     got = ops.gemm_nt_oz(dev(A), dev(B), dev(C0).clone(), alpha=alpha, beta=beta, slices=slices).cpu().numpy()
-    assert np.array_equal(got, want), np.abs(got - want).max()
+    assert np.array_equal(got, want, equal_nan=True), np.nanmax(np.abs(got - want))
+    normal = np.ones((M, N), bool)
+    normal[200:], normal[:, 100:121] = False, False
+    assert np.isfinite(got[normal]).all() and np.isnan(got[220:222]).all() and np.isnan(got[:, 120]).all()
 
 
 def test_auto_picks_slices_by_conditioning(S):

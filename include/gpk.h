@@ -138,6 +138,25 @@ int gpk_kernel_cross_bwd_f32(const gpk_kernel_desc* desc_host, const float* xsg,
                              const float* v, const float* gdiag, float* term_sum, float* grad_xsg, float* grad_xg,
                              int32_t batch, void* stream);
 
+/* fp64 emulation on the INT8 tensor cores (wgmma .s32.s8.s8; Ozaki splitting): every row of an operand is scaled by a
+ * power of two and split error-free into `slices` signed 7-bit integers; the slice products are EXACT in int32 and are
+ * recombined in fp64.  6 slices: 21 int8 GEMMs, product error ~2^-40 |a||b| (zero-mean); 7 slices: 28 GEMMs, ~2^-47.
+ * The fp64 entry points gpk_potrf_f64, gpk_trsm_right_f64, gpk_gemm_nt_f64, gpk_posterior_marginals_f64 and
+ * gpk_sparse_accumulate_f64 take it as three trailing arguments (slices, ws, ws_bytes): slices = 0 keeps every product on
+ * the fp64 tensor cores (ws may be NULL); slices = 5..8 with a caller-owned, 1024-byte aligned scratch `ws` runs the LARGE
+ * GEMM-shaped updates of that call on the int8 tensor cores -- the trailing updates of a factorisation (batch 1,
+ * n_pad >= 2048), and products of batch 1 with M, N, K >= 256 and M N K >= 1.5e9 (reductions longer than 65536 in several
+ * exact passes) -- whenever `ws_bytes` covers them.  Everything else, and every update whose scratch is too small, stays on
+ * the fp64 tensor cores.  The size queries give the scratch that makes every update of a call eligible, 0 when none is:
+ *   gpk_gemm_nt_oz_ws_bytes     one product M x N x K
+ *   gpk_trsm_right_oz_ws_bytes  the largest product of the recursive solve of `rows` right-hand sides (also the solve inside
+ *                               gpk_posterior_marginals_f64 (rows = chunk) and gpk_sparse_accumulate_f64 (rows = c_pad))
+ *   gpk_potrf_oz_ws_bytes       a factorisation (the panel slices; from n_pad >= 4096 those of a pair of panels)
+ * Calls that share a scratch buffer must be stream-ordered with respect to each other. */
+int64_t gpk_gemm_nt_oz_ws_bytes(int64_t M, int64_t N, int64_t K, int32_t slices);
+int64_t gpk_trsm_right_oz_ws_bytes(int64_t n_pad, int64_t rows, int32_t slices);
+int64_t gpk_potrf_oz_ws_bytes(int64_t n_pad, int64_t extra_rows, int32_t slices);
+
 /* GEMM  C = beta*C + alpha * A * B^T   (A: M x K, B: N x K, both K-contiguous; C: M x N).
  * M, N multiples of 128; K a multiple of 16; pointers 16-byte aligned; ld multiples of 2.
  * lower != 0: only tiles with (row tile >= col tile) are touched (SYRK-style trailing update, M >= N).
@@ -145,7 +164,8 @@ int gpk_kernel_cross_bwd_f32(const gpk_kernel_desc* desc_host, const float* xsg,
  * stheno/model/observations.py:301,322,323). */
 int gpk_gemm_nt_f64(int64_t M, int64_t N, int64_t K, double alpha, const double* A, int64_t lda, int64_t a_bstride,
                     const double* B, int64_t ldb, int64_t b_bstride, double beta, double* C, int64_t ldc,
-                    int64_t c_bstride, int32_t lower, int32_t batch, void* stream);
+                    int64_t c_bstride, int32_t lower, int32_t batch, int32_t slices, void* ws, int64_t ws_bytes,
+                    void* stream);
 int gpk_gemm_nt_f32(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t lda, int64_t a_bstride,
                     const float* B, int64_t ldb, int64_t b_bstride, float beta, float* C, int64_t ldc,
                     int64_t c_bstride, int32_t lower, int32_t batch, void* stream);
@@ -157,7 +177,7 @@ int gpk_gemm_nt_f32(int64_t M, int64_t N, int64_t K, float alpha, const float* A
  *   logdet[b] += 2 sum log diag(L) (caller zeroes it); info[b] = first non-positive pivot (1-based) or 0.
  * Replaces B.cholesky + B.logdet: stheno/random.py:274, stheno/model/observations.py:300,334. */
 int gpk_potrf_f64(double* A, int64_t lda, int64_t a_bstride, int64_t n_pad, int64_t extra_rows, double* logdet,
-                  int32_t* info, int32_t batch, void* stream);
+                  int32_t* info, int32_t batch, int32_t slices, void* ws, int64_t ws_bytes, void* stream);
 int gpk_potrf_f32(float* A, int64_t lda, int64_t a_bstride, int64_t n_pad, int64_t extra_rows, float* logdet,
                   int32_t* info, int32_t batch, void* stream);
 
@@ -168,25 +188,9 @@ int gpk_potrf_f32(float* A, int64_t lda, int64_t a_bstride, int64_t n_pad, int64
 int gpk_potrf_f64_tf32x3(double* A, int64_t lda, int64_t a_bstride, int64_t n_pad, int64_t extra_rows, double* logdet,
                          int32_t* info, int32_t batch, float* ws, int64_t ws_elems, void* stream);
 
-/* fp64 emulation on the INT8 tensor cores (wgmma .s32.s8.s8; Ozaki splitting): every row of the panel is scaled by
- * a power of two and split error-free into `slices` signed 7-bit integers; the slice products are EXACT in int32 and are
- * recombined in fp64.  6 slices: 21 int8 GEMMs, product error ~2^-40 |a||b| (zero-mean); 7 slices: 28 GEMMs, ~2^-47.
- * `ws`: 1024-byte aligned workspace of gpk_potrf_oz_ws_bytes(n_pad, extra_rows, slices) bytes.  Same contract as
- * gpk_potrf_f64 otherwise (batch must be 1 for the emulated update; batched problems fall back to the DMMA update). */
-int64_t gpk_potrf_oz_ws_bytes(int64_t n_pad, int64_t extra_rows, int32_t slices);
-int gpk_potrf_f64_oz(double* A, int64_t lda, int64_t a_bstride, int64_t n_pad, int64_t extra_rows, double* logdet,
-                     int32_t* info, int32_t batch, int32_t slices, void* ws, int64_t ws_bytes, void* stream);
-/* Library-wide switch (like cublasSetMathMode), per host thread and device: with slices = 5..8 and a caller-owned, 1024-byte
- * aligned scratch buffer, the LARGE fp64 GEMM-shaped updates inside gpk_potrf_f64 (trailing updates, n_pad >= 2048),
- * gpk_trsm_right_f64 and gpk_gemm_nt_f64 (batch 1, M, N >= 256, M N K >= 1.5e9, K <= 65536) run on the int8 tensor cores
- * whenever the scratch is large enough (gpk_f64_emulation_scratch_bytes for a GEMM, gpk_potrf_oz_ws_bytes for a
- * factorisation); everything else stays on the fp64 tensor cores.  slices = 0 switches it off.  Calls that use the scratch
- * must be stream-ordered with respect to each other. */
-int gpk_set_f64_emulation(int32_t slices, void* scratch, int64_t scratch_bytes);
-int64_t gpk_f64_emulation_scratch_bytes(int64_t M, int64_t N, int64_t K, int32_t slices);
-
-/* The emulated GEMM on its own: C = beta C + alpha A B^T (M % 128 == 0, N % 64 == 0, K % 128 == 0, K <= 65536).
- * `ws`: 1024-byte aligned, >= round_up(gpk_oz_ws_bytes(M, K, slices), 1024) + gpk_oz_ws_bytes(N, K, slices) bytes.
+/* The emulated GEMM on its own, whatever its size: C = beta C + alpha A B^T (M % 128 == 0, N % 64 == 0, K a positive
+ * multiple of 128), slices = 5..8.  `ws`: 1024-byte aligned, >= round_up(gpk_oz_ws_bytes(M, K, slices), 1024) +
+ * gpk_oz_ws_bytes(N, K, slices) bytes.
  * Rows of every finite magnitude are scaled exactly (subnormal to near overflow); a row of A (B) holding a NaN or an
  * infinity makes its row (column) of alpha A B^T NaN, where fp64 gives NaN or +-inf.  Lower mode and beta as in
  * gpk_gemm_nt_f64: only the tiles that touch the lower triangle are read or written, for every beta. */
@@ -199,7 +203,8 @@ int gpk_gemm_nt_f64_oz(int64_t M, int64_t N, int64_t K, double alpha, const doub
  * Row r of the result is (L^-1 b_r)^T.  Replaces B.solve(L, .) / B.iqf:  stheno/model/observations.py:301 and
  * the PosteriorMean / PosteriorKernel evaluation behind observations.py:143-168. */
 int gpk_trsm_right_f64(const double* L, int64_t ldl, int64_t l_bstride, int64_t n_pad, double* B, int64_t ldb,
-                       int64_t b_bstride, int64_t rows, int32_t batch, void* stream);
+                       int64_t b_bstride, int64_t rows, int32_t batch, int32_t slices, void* ws, int64_t ws_bytes,
+                       void* stream);
 int gpk_trsm_right_f32(const float* L, int64_t ldl, int64_t l_bstride, int64_t n_pad, float* B, int64_t ldb,
                        int64_t b_bstride, int64_t rows, int32_t batch, void* stream);
 
@@ -252,7 +257,7 @@ int gpk_transpose_f32(const float* src, int64_t lds, int64_t s_bstride, int64_t 
 int gpk_posterior_marginals_f64(const gpk_kernel_desc* desc_host, const double* xsg, int64_t xsg_gstride, int64_t m,
                                 const double* xg, int64_t xg_gstride, int64_t n, int32_t d, const double* L, int64_t ldl,
                                 int64_t n_pad, const double* half_y, double* dot, double* sq, int64_t chunk, double* ws,
-                                int64_t ws_elems, void* stream);
+                                int64_t ws_elems, int32_t slices, void* oz_ws, int64_t oz_ws_bytes, void* stream);
 int gpk_posterior_marginals_f32(const gpk_kernel_desc* desc_host, const float* xsg, int64_t xsg_gstride, int64_t m,
                                 const float* xg, int64_t xg_gstride, int64_t n, int32_t d, const float* L, int64_t ldl,
                                 int64_t n_pad, const float* half_y, float* dot, float* sq, int64_t chunk, float* ws,
@@ -267,14 +272,14 @@ int gpk_posterior_marginals_f32(const gpk_kernel_desc* desc_host, const float* x
  *   prod += W diag(1/kn) ybar  (:327);  scalars[0] += sum log(2 pi kn_i) (:334);  scalars[1] += sum ybar_i^2 / kn_i (:335)
  * xg / zg: pre-stretched inputs [n_groups][c or m][d] (group strides given); Lz: padded lower factor of K_z + eps I
  * (gpk_potrf); ws: 16-byte aligned workspace of gpk_sparse_ws_elems(c, m_pad) elements.  The m^2 c flops of the solve and of
- * the accumulation run on the tensor cores (the int8 emulation when gpk_set_f64_emulation is on and its scratch fits
- * gpk_f64_emulation_scratch_bytes(m_pad, m_pad, c_pad) and the solve's largest product). */
+ * the accumulation run on the tensor cores (the int8 emulation of those (slices, oz_ws, oz_ws_bytes) admits:
+ * gpk_gemm_nt_oz_ws_bytes(m_pad, m_pad, c_pad) covers the accumulation, gpk_trsm_right_oz_ws_bytes(m_pad, c_pad) the solve). */
 int64_t gpk_sparse_ws_elems(int64_t c, int64_t m_pad);
 int gpk_sparse_accumulate_f64(const gpk_kernel_desc* desc_host, const double* xg, int64_t xg_gstride, int64_t c,
                               const double* zg, int64_t zg_gstride, int64_t m, int32_t d, const double* Lz, int64_t ldl,
                               int64_t m_pad, const double* kdiag, const double* kn, const double* ybar, int32_t method,
                               double* A, int64_t lda, double* prod, double* scalars, double* ws, int64_t ws_elems,
-                              void* stream);
+                              int32_t slices, void* oz_ws, int64_t oz_ws_bytes, void* stream);
 int gpk_sparse_accumulate_f32(const gpk_kernel_desc* desc_host, const float* xg, int64_t xg_gstride, int64_t c,
                               const float* zg, int64_t zg_gstride, int64_t m, int32_t d, const float* Lz, int64_t ldl,
                               int64_t m_pad, const float* kdiag, const float* kn, const float* ybar, int32_t method, float* A,

@@ -33,7 +33,8 @@ class KernelDesc(Structure):
 
 _i32, _i64, _f64, _f32, _ptr = c_int32, c_int64, c_double, c_float, c_void_p
 
-# name -> argtypes (restype int unless listed in _RESTYPES); {T} = scalar type of the suffix (alpha / beta)
+# name -> argtypes of name_f64 / name_f32 (restype int): "T" = the scalar type of the suffix (alpha / beta); "OZ" = the
+# int8-slice emulation arguments (slices, ws, ws_bytes) that only the fp64 entry points take
 _SIGNATURES = {
     "gpk_kernel_matrix": [POINTER(KernelDesc), _ptr, _i64, _i64, _i64, _ptr, _i64, _i64, _i64, _i32, _f64, _ptr, _i64,
                           _f64, _i32, _ptr, _i64, _i64, _i32, _ptr],
@@ -43,9 +44,9 @@ _SIGNATURES = {
                               _ptr],
     "gpk_kernel_cross_bwd": [POINTER(KernelDesc), _ptr, _i64, _i64, _i64, _ptr, _i64, _i64, _i64, _i32, _ptr, _i64, _i64,
                              _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr],
-    "gpk_gemm_nt": [_i64, _i64, _i64, "T", _ptr, _i64, _i64, _ptr, _i64, _i64, "T", _ptr, _i64, _i64, _i32, _i32, _ptr],
-    "gpk_potrf": [_ptr, _i64, _i64, _i64, _i64, _ptr, _ptr, _i32, _ptr],
-    "gpk_trsm_right": [_ptr, _i64, _i64, _i64, _ptr, _i64, _i64, _i64, _i32, _ptr],
+    "gpk_gemm_nt": [_i64, _i64, _i64, "T", _ptr, _i64, _i64, _ptr, _i64, _i64, "T", _ptr, _i64, _i64, _i32, _i32, "OZ", _ptr],
+    "gpk_potrf": [_ptr, _i64, _i64, _i64, _i64, _ptr, _ptr, _i32, "OZ", _ptr],
+    "gpk_trsm_right": [_ptr, _i64, _i64, _i64, _ptr, _i64, _i64, _i64, _i32, "OZ", _ptr],
     "gpk_trsm_right_t": [_ptr, _i64, _i64, _i64, _ptr, _i64, _i64, _i64, _i32, _ptr],
     "gpk_logpdf_finish": [_ptr, _i64, _i64, _i64, _i64, _i32, _ptr, _ptr, _i32, _ptr],
     "gpk_row_dot_sq": [_ptr, _i64, _i64, _i64, _i64, _ptr, _i64, _ptr, _ptr, _i64, _i32, _ptr],
@@ -53,9 +54,9 @@ _SIGNATURES = {
     "gpk_symmetrize": [_ptr, _i64, _i64, _i64, _i32, _ptr],
     "gpk_transpose": [_ptr, _i64, _i64, _i64, _i64, _ptr, _i64, _i64, _i32, _ptr],
     "gpk_posterior_marginals": [POINTER(KernelDesc), _ptr, _i64, _i64, _ptr, _i64, _i64, _i32, _ptr, _i64, _i64, _ptr, _ptr, _ptr,
-                                _i64, _ptr, _i64, _ptr],
+                                _i64, _ptr, _i64, "OZ", _ptr],
     "gpk_sparse_accumulate": [POINTER(KernelDesc), _ptr, _i64, _i64, _ptr, _i64, _i64, _i32, _ptr, _i64, _i64, _ptr, _ptr, _ptr,
-                              _i32, _ptr, _i64, _ptr, _ptr, _ptr, _i64, _ptr],
+                              _i32, _ptr, _i64, _ptr, _ptr, _ptr, _i64, "OZ", _ptr],
 }
 _PLAIN = {
     "gpk_version": ([], c_int32),
@@ -68,10 +69,9 @@ _PLAIN = {
     "gpk_launch_count_reset": ([], None),
     "gpk_potrf_f64_tf32x3": ([_ptr, _i64, _i64, _i64, _i64, _ptr, _ptr, _i32, _ptr, _i64, _ptr], c_int32),
     "gpk_potrf_oz_ws_bytes": ([_i64, _i64, _i32], _i64),
-    "gpk_potrf_f64_oz": ([_ptr, _i64, _i64, _i64, _i64, _ptr, _ptr, _i32, _i32, _ptr, _i64, _ptr], c_int32),
+    "gpk_trsm_right_oz_ws_bytes": ([_i64, _i64, _i32], _i64),
+    "gpk_gemm_nt_oz_ws_bytes": ([_i64, _i64, _i64, _i32], _i64),
     "gpk_oz_ws_bytes": ([_i64, _i64, _i32], _i64),
-    "gpk_set_f64_emulation": ([_i32, _ptr, _i64], c_int32),
-    "gpk_f64_emulation_scratch_bytes": ([_i64, _i64, _i64, _i32], _i64),
     "gpk_gemm_nt_f64_oz": ([_i64, _i64, _i64, _f64, _ptr, _i64, _ptr, _i64, _f64, _ptr, _i64, _i32, _i32, _ptr, _i64,
                             _ptr], c_int32),
     "gpk_gemm_profile_enable": ([_i32], None),
@@ -98,9 +98,9 @@ def load(build_if_missing=True):
         raise RuntimeError(f"{LIB_PATH} is missing: the CUDA extension has not been built (no CPU fallback exists)")
     lib = ctypes.CDLL(LIB_PATH)
     for name, args in _SIGNATURES.items():
-        for suf, scalar in (("f64", c_double), ("f32", c_float)):
+        for suf, scalar, oz in (("f64", c_double, [_i32, _ptr, _i64]), ("f32", c_float, [])):
             fn = getattr(lib, f"{name}_{suf}")
-            fn.argtypes = [scalar if a == "T" else a for a in args]
+            fn.argtypes = [t for a in args for t in (oz if a == "OZ" else [scalar] if a == "T" else [a])]
             fn.restype = c_int32
     for name, (args, res) in _PLAIN.items():
         fn = getattr(lib, name)

@@ -125,13 +125,9 @@ __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double
                : "d"(a), "d"(b));
 }
 
-// fp64 emulation mode set by the caller through gpk_set_f64_emulation (gemm_oz.cu), per host thread and device
-struct Emulation {
-  int32_t slices = 0;
-  void* scratch = nullptr;
-  int64_t bytes = 0;
-};
-Emulation& emulation();
+// The int8-slice emulation arguments (slices, ws, ws_bytes) of the fp64 entry points: slices 0 (fp64 tensor cores) or 5..8
+// with a 1024-byte aligned scratch.  0 or GPK_ERR_ARG (gemm_oz.cu).
+int oz_check_emulation(int32_t slices, const void* ws);
 
 template <typename T>
 __device__ __forceinline__ T warp_sum(T v) {

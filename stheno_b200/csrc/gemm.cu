@@ -11,7 +11,7 @@
 //   fragment load is one conflict-free, warp-contiguous LDS.128 that feeds TWO DMMAs (the even-k one and the odd-k one --
 //   the k order inside a k-group of 8 is permuted identically for A and B, which leaves the product unchanged).
 //   Roofline: fp64 tensor pipe (measured 37.1 TFLOP/s DMMA peak); algorithmic flops 2 M N K (M N K for lower).
-//   Large batch-1 products go to the int8-slice emulation (gemm_oz.cu) instead when the caller enabled it.
+//   Large batch-1 products go to the int8-slice emulation (gemm_oz.cu) instead when the caller passes its slices and scratch.
 // fp32: the 3xTF32 wgmma kernel (gemm_tc32.cu) where its shape rules allow, else a register-tiled FFMA kernel (8 x 8
 //   micro-tiles), double-buffered.
 #include <vector>
@@ -480,16 +480,17 @@ void prof_begin(cudaStream_t s, double flops, int kind = 0) {
 void prof_end(cudaStream_t s) { cudaEventRecord(g_prof.ev.back(), s); }
 
 int gemm_nt_f64_emulated(int64_t, int64_t, int64_t, double, const double*, int64_t, const double*, int64_t, double, double*,
-                         int64_t, int32_t, cudaStream_t);  // gemm_oz.cu: 1 = done, 0 = not applicable, < 0 error
+                         int64_t, int32_t, int32_t, void*, int64_t, cudaStream_t);  // gemm_oz.cu: 1 = done, 0 = not applicable, < 0 error
 
 int gemm_nt_f64(int64_t M, int64_t N, int64_t K, double alpha, const double* A, int64_t lda, int64_t a_bs,
                 const double* B, int64_t ldb, int64_t b_bs, double beta, double* C, int64_t ldc, int64_t c_bs,
-                int32_t lower, int32_t batch, cudaStream_t stream) {
+                int32_t lower, int32_t batch, int32_t slices, void* ws, int64_t ws_bytes, cudaStream_t stream) {
   int rc = check_gemm_args<double>(M, N, K, A, lda, B, ldb, C, ldc, batch);
+  if (!rc) rc = oz_check_emulation(slices, ws);
   if (rc) return rc;
   if (M == 0 || N == 0) return 0;
-  if (batch == 1 && K >= 256) {  // large updates: int8-slice emulation on wgmma when the caller enabled it
-    rc = gemm_nt_f64_emulated(M, N, K, alpha, A, lda, B, ldb, beta, C, ldc, lower, stream);
+  if (batch == 1 && slices) {  // large updates: int8-slice emulation on wgmma when the caller asked for it
+    rc = gemm_nt_f64_emulated(M, N, K, alpha, A, lda, B, ldb, beta, C, ldc, lower, slices, ws, ws_bytes, stream);
     if (rc < 0) return rc;
     if (rc == 1) return 0;
   }
@@ -598,9 +599,10 @@ int gpk_gemm_profile_read_kind(int32_t kind, double* total_ms, double* total_flo
 }
 int gpk_gemm_nt_f64(int64_t M, int64_t N, int64_t K, double alpha, const double* A, int64_t lda, int64_t a_bstride,
                     const double* B, int64_t ldb, int64_t b_bstride, double beta, double* C, int64_t ldc,
-                    int64_t c_bstride, int32_t lower, int32_t batch, void* stream) {
+                    int64_t c_bstride, int32_t lower, int32_t batch, int32_t slices, void* ws, int64_t ws_bytes,
+                    void* stream) {
   return gpk::gemm_nt_f64(M, N, K, alpha, A, lda, a_bstride, B, ldb, b_bstride, beta, C, ldc, c_bstride, lower, batch,
-                          (cudaStream_t)stream);
+                          slices, ws, ws_bytes, (cudaStream_t)stream);
 }
 int gpk_gemm_nt_f32(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t lda, int64_t a_bstride,
                     const float* B, int64_t ldb, int64_t b_bstride, float beta, float* C, int64_t ldc,

@@ -577,67 +577,63 @@ int oz_gemm_sliced(int64_t M, int64_t N, int64_t K, double alpha, const void* ws
   return GPK_ERR_ARG;
 }
 
-// ---- library-wide fp64 emulation mode (like cublasSetMathMode): set per host thread and device by the caller, who also
-// owns the scratch buffer.  Work that uses the scratch must be stream-ordered (one stream at a time per host thread). ----
-Emulation& emulation() {
-  static thread_local Emulation em[64];
-  int dev = 0;
-  cudaGetDevice(&dev);
-  return em[(dev < 0 || dev >= 64) ? 0 : dev];
+int oz_check_emulation(int32_t S, const void* ws) {
+  if (S == 0) return 0;
+  return (S < 5 || S > 8 || !ws || reinterpret_cast<uintptr_t>(ws) % 1024) ? GPK_ERR_ARG : 0;
 }
 
 static inline int64_t round_up_1k(int64_t x) { return (x + 1023) & ~int64_t(1023); }
 
-int64_t oz_gemm_scratch_bytes(int64_t M, int64_t N, int64_t K, int32_t S) {
-  return round_up_1k(oz_ws_bytes(M, K, S)) + oz_ws_bytes(N, K, S);
+// int32 accumulation is exact for K <= 65536 per pass: longer reductions (the sparse path's n = 262144) run as several
+// passes over K chunks of this length (a multiple of 128; the last chunk is the remainder), each adding into C
+static int64_t oz_k_chunk(int64_t K) {
+  const int64_t passes = K > 65536 ? (K + 65535) / 65536 : 1;
+  return ((K / passes + 127) / 128) * 128;
+}
+
+// scratch of an emulated GEMM with K chunks of kc: A's slices, then (unless B is A) B's from the next 1024-byte boundary
+static int64_t oz_gemm_need(int64_t M, int64_t N, int64_t kc, int32_t S, bool same) {
+  return same ? oz_ws_bytes(M, kc, S) : round_up_1k(oz_ws_bytes(M, kc, S)) + oz_ws_bytes(N, kc, S);
+}
+
+// C = beta C + alpha A B^T on the int8 tensor cores, K chunk by K chunk; `ws` holds oz_gemm_need bytes
+static int oz_gemm(int64_t M, int64_t N, int64_t K, double alpha, const double* A, int64_t lda, const double* B, int64_t ldb,
+                   double beta, double* C, int64_t ldc, int32_t lower, int32_t S, void* ws, bool same, cudaStream_t stream) {
+  const int64_t kc = oz_k_chunk(K);
+  void* wsb = static_cast<char*>(ws) + (same ? 0 : round_up_1k(oz_ws_bytes(M, kc, S)));
+  int rc;
+  for (int64_t k0 = 0; k0 < K; k0 += kc) {
+    const int64_t kk = (K - k0 < kc) ? K - k0 : kc;
+    if ((rc = oz_slice_panel(A + k0, lda, M, kk, ws, M, S, stream))) return rc;
+    if (!same && (rc = oz_slice_panel(B + k0, ldb, N, kk, wsb, N, S, stream))) return rc;
+    if ((rc = oz_gemm_sliced(M, N, kk, alpha, ws, M, 0, same ? ws : wsb, same ? M : N, 0, k0 == 0 ? beta : 1.0, C, ldc, lower,
+                             S, stream)))
+      return rc;
+  }
+  return 0;
 }
 
 // 1 = done on the emulated path, 0 = not applicable (caller uses DMMA), < 0 = error
 int gemm_nt_f64_emulated(int64_t M, int64_t N, int64_t K, double alpha, const double* A, int64_t lda, const double* B,
-                         int64_t ldb, double beta, double* C, int64_t ldc, int32_t lower, cudaStream_t stream) {
-  const Emulation& em = emulation();
-  if (em.slices < 5 || em.slices > 8 || !em.scratch) return 0;
+                         int64_t ldb, double beta, double* C, int64_t ldc, int32_t lower, int32_t S, void* ws, int64_t ws_bytes,
+                         cudaStream_t stream) {
+  if (!gpk_gemm_nt_oz_ws_bytes(M, N, K, S)) return 0;
   if (M % OZ_BM || N % OZ_BN || K % 128 || lda % 2 || ldb % 2 || ldc % 2) return 0;
   if ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B) | reinterpret_cast<uintptr_t>(C)) % 16) return 0;
-  // worth it only when the product dwarfs the slicing passes and fills the machine
-  if (M < 256 || N < 256 || (double)M * (double)N * (double)K < 1.5e9) return 0;
   const bool same = (A == B && lda == ldb && M >= N);
-  // int32 accumulation is exact for K <= 65536 per pass: longer reductions (the sparse path's n = 262144) run as several
-  // passes over K chunks, each adding into C
-  constexpr int64_t KC_MAX = 65536;
-  const int64_t passes = (K + KC_MAX - 1) / KC_MAX;
-  const int64_t kc = ((K / passes + 127) / 128) * 128;  // chunk length (multiple of 128), last chunk = remainder
-  const int64_t off_b = same ? 0 : round_up_1k(oz_ws_bytes(M, kc, em.slices));
-  if (em.bytes < off_b + oz_ws_bytes(same ? M : N, kc, em.slices)) return 0;
-  int rc;
-  void* wsa = em.scratch;
-  void* wsb = static_cast<char*>(em.scratch) + off_b;
-  for (int64_t k0 = 0; k0 < K; k0 += kc) {
-    const int64_t kk = (K - k0 < kc) ? K - k0 : kc;
-    if ((rc = oz_slice_panel(A + k0, lda, M, kk, wsa, M, em.slices, stream))) return rc;
-    if (!same && (rc = oz_slice_panel(B + k0, ldb, N, kk, wsb, N, em.slices, stream))) return rc;
-    if ((rc = oz_gemm_sliced(M, N, kk, alpha, wsa, M, 0, same ? wsa : wsb, same ? M : N, 0, k0 == 0 ? beta : 1.0, C, ldc, lower,
-                             em.slices, stream)))
-      return rc;
-  }
-  return 1;
+  if (ws_bytes < oz_gemm_need(M, N, oz_k_chunk(K), S, same)) return 0;
+  const int rc = oz_gemm(M, N, K, alpha, A, lda, B, ldb, beta, C, ldc, lower, S, ws, same, stream);
+  return rc < 0 ? rc : 1;
 }
 
 }  // namespace gpk
 
 extern "C" {
 
-int gpk_set_f64_emulation(int32_t slices, void* scratch, int64_t scratch_bytes) {
-  if (slices != 0 && (slices < 5 || slices > 8)) return GPK_ERR_ARG;
-  if (slices != 0 && (!scratch || reinterpret_cast<uintptr_t>(scratch) % 1024 || scratch_bytes <= 0)) return GPK_ERR_ARG;
-  gpk::Emulation& em = gpk::emulation();
-  em.slices = slices;
-  em.scratch = slices ? scratch : nullptr;
-  em.bytes = slices ? scratch_bytes : 0;
-  return 0;
-}
-int64_t gpk_f64_emulation_scratch_bytes(int64_t M, int64_t N, int64_t K, int32_t slices) {
-  return gpk::oz_gemm_scratch_bytes(M, N, K, slices);
+int64_t gpk_gemm_nt_oz_ws_bytes(int64_t M, int64_t N, int64_t K, int32_t slices) {
+  // worth it only when the product dwarfs the slicing passes and fills the machine
+  if (slices < 5 || slices > 8 || M < 256 || N < 256 || K < 256 || (double)M * (double)N * (double)K < 1.5e9) return 0;
+  return gpk::oz_gemm_need(M, N, gpk::oz_k_chunk(K), slices, false);
 }
 
 int64_t gpk_oz_ws_bytes(int64_t rows, int64_t K, int32_t slices) { return gpk::oz_ws_bytes(rows, K, slices); }
@@ -666,17 +662,11 @@ int32_t gpk_debug_oz_tile(int32_t lower, int32_t tiles_m, int32_t tiles_n, int32
 int gpk_gemm_nt_f64_oz(int64_t M, int64_t N, int64_t K, double alpha, const double* A, int64_t lda, const double* B,
                        int64_t ldb, double beta, double* C, int64_t ldc, int32_t lower, int32_t slices, void* ws,
                        int64_t ws_bytes, void* stream) {
-  if (slices < 5 || slices > 8 || !ws) return GPK_ERR_ARG;
-  const int64_t need_a = gpk::oz_ws_bytes(M, K, slices), need_b = gpk::oz_ws_bytes(N, K, slices);
   const bool same = (A == B && lda == ldb && M >= N);
-  const int64_t off_b = same ? 0 : ((need_a + 1023) & ~int64_t(1023));
-  if (ws_bytes < off_b + (same ? need_a : need_b) || reinterpret_cast<uintptr_t>(ws) % 1024) return GPK_ERR_ARG;
-  cudaStream_t s = (cudaStream_t)stream;
-  int rc;
-  void* wsb = static_cast<char*>(ws) + off_b;
-  if ((rc = gpk::oz_slice_panel(A, lda, M, K, ws, M, slices, s))) return rc;
-  if (!same && (rc = gpk::oz_slice_panel(B, ldb, N, K, wsb, N, slices, s))) return rc;
-  return gpk::oz_gemm_sliced(M, N, K, alpha, ws, M, 0, same ? ws : wsb, same ? M : N, 0, beta, C, ldc, lower, slices, s);
+  if (slices == 0 || gpk::oz_check_emulation(slices, ws) || K <= 0 ||
+      ws_bytes < gpk::oz_gemm_need(M, N, gpk::oz_k_chunk(K), slices, same))
+    return GPK_ERR_ARG;
+  return gpk::oz_gemm(M, N, K, alpha, A, lda, B, ldb, beta, C, ldc, lower, slices, ws, same, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -9,7 +9,7 @@
 //                (3) gemm (K=128): update of the rest of the outer panel
 //              and per outer panel one big SYRK-style trailing update (K = 512), which carries > 90 % of the n^3/3 flops
 //              at n = 16384 with C read/written once per 512 columns: on the int8 tensor cores (fp64 emulated with exact
-//              integer slice products, gemm_oz.cu) when the caller enabled it, on the fp64 tensor cores (DMMA) otherwise
+//              integer slice products, gemm_oz.cu) when the caller passes its slices, on the fp64 tensor cores (DMMA) otherwise
 //              (measured: 512 beats 256, 768, 1024 for both).  Emulated path, n_pad >= 4096: the FAR part of the trailing
 //              matrix is updated once per PAIR of panels with K = 1024 (potrf_driver_pairs): half the passes over the
 //              trailing matrix and half the accumulator drains per flop, the panels themselves unchanged.
@@ -30,18 +30,19 @@
 namespace gpk {
 
 int gemm_nt_f64(int64_t, int64_t, int64_t, double, const double*, int64_t, int64_t, const double*, int64_t, int64_t,
-                double, double*, int64_t, int64_t, int32_t, int32_t, cudaStream_t);
+                double, double*, int64_t, int64_t, int32_t, int32_t, int32_t, void*, int64_t, cudaStream_t);
 int gemm_nt_f32(int64_t, int64_t, int64_t, float, const float*, int64_t, int64_t, const float*, int64_t, int64_t,
                 float, float*, int64_t, int64_t, int32_t, int32_t, cudaStream_t);
 
+// (S, ws, ws_bytes): the int8-slice emulation the caller asked for (gpk.h); fp32 has none
 static inline int gemm_nt(int64_t M, int64_t N, int64_t K, double alpha, const double* A, int64_t lda, int64_t a_bs,
                           const double* B, int64_t ldb, int64_t b_bs, double beta, double* C, int64_t ldc, int64_t c_bs,
-                          int32_t lower, int32_t batch, cudaStream_t s) {
-  return gemm_nt_f64(M, N, K, alpha, A, lda, a_bs, B, ldb, b_bs, beta, C, ldc, c_bs, lower, batch, s);
+                          int32_t lower, int32_t batch, int32_t S, void* ws, int64_t ws_bytes, cudaStream_t s) {
+  return gemm_nt_f64(M, N, K, alpha, A, lda, a_bs, B, ldb, b_bs, beta, C, ldc, c_bs, lower, batch, S, ws, ws_bytes, s);
 }
 static inline int gemm_nt(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t lda, int64_t a_bs,
                           const float* B, int64_t ldb, int64_t b_bs, float beta, float* C, int64_t ldc, int64_t c_bs,
-                          int32_t lower, int32_t batch, cudaStream_t s) {
+                          int32_t lower, int32_t batch, int32_t, void*, int64_t, cudaStream_t s) {
   return gemm_nt_f32(M, N, K, alpha, A, lda, a_bs, B, ldb, b_bs, beta, C, ldc, c_bs, lower, batch, s);
 }
 
@@ -698,7 +699,7 @@ static int factor_panel(T* A, int64_t lda, int64_t a_bs, int64_t R, int64_t kb, 
       const int64_t ncols = ke - (j + NB);
       if (ncols > 0) {
         if ((rc = gemm_nt(below, ncols, (int64_t)NB, T(-1), A21, lda, a_bs, A21, lda, a_bs, T(1),
-                          A + (j + NB) * lda + (j + NB), lda, a_bs, 1, batch, stream)))
+                          A + (j + NB) * lda + (j + NB), lda, a_bs, 1, batch, 0, nullptr, 0, stream)))
           return rc;
       }
     }
@@ -742,7 +743,7 @@ static int factor_panel_split(T* A, int64_t lda, int64_t a_bs, int64_t R, int64_
         if ((rc = ce(cudaStreamWaitEvent(la.bulk, la.crit, 0)))) return rc;
         // rows [b0, R) x columns [j1, ke) of the panel -= X[b0:, j] X[j1:ke, j]^T
         if ((rc = gemm_nt(brows, ke - j1, (int64_t)NB, T(-1), A + b0 * lda + j, lda, a_bs, X1, lda, a_bs, T(1),
-                          A + b0 * lda + j1, lda, a_bs, 0, batch, la.bulk)))
+                          A + b0 * lda + j1, lda, a_bs, 0, batch, 0, nullptr, 0, la.bulk)))
           return rc;
         if ((rc = ce(cudaEventRecord(la.bulk_done, la.bulk)))) return rc;
         bulk_pending = true;
@@ -766,7 +767,6 @@ int64_t oz_ws_bytes(int64_t rows, int64_t K, int32_t S);  // gemm_oz.cu
 int oz_slice_panel(const double*, int64_t, int64_t, int64_t, void*, int64_t, int32_t, cudaStream_t);
 int oz_gemm_sliced(int64_t, int64_t, int64_t, double, const void*, int64_t, int64_t, const void*, int64_t, int64_t, double,
                    double*, int64_t, int32_t, int32_t, cudaStream_t);
-// (Emulation / emulation(): common.cuh -- the caller's gpk_set_f64_emulation state for this host thread / device)
 
 // How the K = NB_OUTER trailing updates of an fp64 factorisation are formed:
 //   MODE_F64     fp64 tensor cores (DMMA) straight from the matrix
@@ -815,7 +815,7 @@ int prepare_panel<double>(const Trailing& t, const double* P, int64_t ldp, int64
 template <typename T>
 static int trailing_update(int used, const Trailing&, int64_t rA, int64_t rB, int64_t M, int64_t N, int64_t K, const T* PA,
                            const T* PB, int64_t lda, int64_t a_bs, T* C, int32_t lower, int32_t batch, cudaStream_t stream) {
-  return gemm_nt(M, N, K, T(-1), PA, lda, a_bs, PB, lda, a_bs, T(1), C, lda, a_bs, lower, batch, stream);
+  return gemm_nt(M, N, K, T(-1), PA, lda, a_bs, PB, lda, a_bs, T(1), C, lda, a_bs, lower, batch, 0, nullptr, 0, stream);
 }
 template <>
 int trailing_update<double>(int used, const Trailing& t, int64_t rA, int64_t rB, int64_t M, int64_t N, int64_t K,
@@ -825,7 +825,7 @@ int trailing_update<double>(int used, const Trailing& t, int64_t rA, int64_t rB,
     return syrk_f64_tf32x3(M, N, K, static_cast<const float*>(t.ws) + rA * K, C, lda, stream);
   if (used == MODE_OZAKI)
     return oz_gemm_sliced(M, N, K, -1.0, t.ws, t.cap_rows, rA, t.ws, t.cap_rows, rB, 1.0, C, lda, lower, t.slices, stream);
-  return gemm_nt(M, N, K, -1.0, PA, lda, a_bs, PB, lda, a_bs, 1.0, C, lda, a_bs, lower, batch, stream);
+  return gemm_nt(M, N, K, -1.0, PA, lda, a_bs, PB, lda, a_bs, 1.0, C, lda, a_bs, lower, batch, 0, nullptr, 0, stream);
 }
 
 // ---- fp64 + int8 emulation, single matrix: outer panels factorised in PAIRS ------------------------------------------
@@ -904,25 +904,7 @@ static int potrf_driver(T* A, int64_t lda, int64_t a_bs, int64_t n_pad, int64_t 
   if (n_pad % NB || extra_rows % NB || lda < n_pad) return GPK_ERR_ARG;
   if (lda % (16 / sizeof(T)) || reinterpret_cast<uintptr_t>(A) % 16) return GPK_ERR_ALIGN;
   const int64_t R = n_pad + extra_rows;
-  if (tr.mode == MODE_F64 && sizeof(T) == 8 && batch == 1 && n_pad >= 2048) {
-    // the caller enabled the int8-slice emulation (gpk_set_f64_emulation) and its scratch holds this panel's slices
-    const Emulation& em = emulation();
-    if (em.slices >= 5 && em.slices <= 8 && em.scratch && em.bytes >= oz_ws_bytes(R, NB_OUTER, em.slices)) {
-      tr.mode = MODE_OZAKI;
-      tr.ws = em.scratch;
-      tr.ws_bytes = em.bytes;
-      tr.slices = em.slices;
-    }
-  }
   tr.cap_rows = R;
-  // Inside the factorisation the scratch belongs to the panel slices, and updates are enqueued on several streams at once:
-  // the generic GEMM entry must not pick the emulated path (and the scratch) on its own while this driver enqueues work.
-  struct SuspendEmulation {
-    Emulation& em;
-    int32_t saved;
-    explicit SuspendEmulation(Emulation& e) : em(e), saved(e.slices) { em.slices = 0; }
-    ~SuspendEmulation() { em.slices = saved; }
-  } suspend(emulation());
   int rc;
   Lookahead& la = lookahead();
   if (tr.mode == MODE_OZAKI && sizeof(T) == 8 && batch == 1 && la.ok && n_pad >= 4096 &&
@@ -982,30 +964,33 @@ static int potrf_driver(T* A, int64_t lda, int64_t a_bs, int64_t n_pad, int64_t 
   return 0;
 }
 
-// X L^T = B, recursive halving (all sizes multiples of 128).
+// X L^T = B, recursive halving (all sizes multiples of 128): the first h columns, the GEMM, then the last n - h columns.
+static inline int64_t trsm_split(int64_t n) { return ((n / NB) / 2) * NB; }
+
 template <typename T>
 static int trsm_right_rec(const T* L, int64_t ldl, int64_t l_bs, int64_t n, T* B, int64_t ldb, int64_t b_bs,
-                          int64_t rows, int32_t batch, cudaStream_t stream) {
+                          int64_t rows, int32_t batch, int32_t S, void* ws, int64_t ws_bytes, cudaStream_t stream) {
   if (n <= 0) return 0;
   if (n == NB) return trsm_leaf_fwd<T>(L, ldl, l_bs, B, ldb, b_bs, rows, batch, stream);
-  const int64_t h = ((n / NB) / 2) * NB;
+  const int64_t h = trsm_split(n);
   int rc;
-  if ((rc = trsm_right_rec<T>(L, ldl, l_bs, h, B, ldb, b_bs, rows, batch, stream))) return rc;
-  if ((rc = gemm_nt(rows, n - h, h, T(-1), B, ldb, b_bs, L + h * ldl, ldl, l_bs, T(1), B + h, ldb, b_bs, 0, batch,
-                    stream)))
+  if ((rc = trsm_right_rec<T>(L, ldl, l_bs, h, B, ldb, b_bs, rows, batch, S, ws, ws_bytes, stream))) return rc;
+  if ((rc = gemm_nt(rows, n - h, h, T(-1), B, ldb, b_bs, L + h * ldl, ldl, l_bs, T(1), B + h, ldb, b_bs, 0, batch, S, ws,
+                    ws_bytes, stream)))
     return rc;
-  return trsm_right_rec<T>(L + h * ldl + h, ldl, l_bs, n - h, B + h, ldb, b_bs, rows, batch, stream);
+  return trsm_right_rec<T>(L + h * ldl + h, ldl, l_bs, n - h, B + h, ldb, b_bs, rows, batch, S, ws, ws_bytes, stream);
 }
 
 template <typename T>
 static int trsm_right_driver(const T* L, int64_t ldl, int64_t l_bs, int64_t n_pad, T* B, int64_t ldb, int64_t b_bs,
-                             int64_t rows, int32_t batch, cudaStream_t stream) {
+                             int64_t rows, int32_t batch, int32_t S, void* ws, int64_t ws_bytes, cudaStream_t stream) {
   if (!L || !B || n_pad < 0 || rows < 0 || batch < 1) return GPK_ERR_ARG;
   if (n_pad % NB || rows % NB || ldl < n_pad || ldb < n_pad) return GPK_ERR_ARG;
   if (ldl % (16 / sizeof(T)) || ldb % (16 / sizeof(T))) return GPK_ERR_ALIGN;
   if ((reinterpret_cast<uintptr_t>(L) | reinterpret_cast<uintptr_t>(B)) % 16) return GPK_ERR_ALIGN;
+  if (const int rc = oz_check_emulation(S, ws)) return rc;
   if (rows == 0) return 0;
-  return trsm_right_rec<T>(L, ldl, l_bs, n_pad, B, ldb, b_bs, rows, batch, stream);
+  return trsm_right_rec<T>(L, ldl, l_bs, n_pad, B, ldb, b_bs, rows, batch, S, ws, ws_bytes, stream);
 }
 
 // X L = B (backward substitution), right-looking over 128-blocks from the last to the first.  The off-diagonal
@@ -1059,13 +1044,31 @@ int gpk_debug_leaf_phase_clock(void* buf16_int64) {
   return e == cudaSuccess ? 0 : -1000 - (int)e;
 }
 int64_t gpk_potrf_oz_ws_bytes(int64_t n_pad, int64_t extra_rows, int32_t slices) {
+  if (slices < 5 || slices > 8 || n_pad < 2048) return 0;
   const int64_t one = gpk::oz_ws_bytes(n_pad + extra_rows, gpk::NB_OUTER, slices);
   const int64_t pairs = gpk::potrf_pairs_ws_bytes(n_pad + extra_rows, slices);  // the pair scheme (n_pad >= 4096)
   return n_pad >= 4096 && pairs > one ? pairs : one;
 }
+int64_t gpk_trsm_right_oz_ws_bytes(int64_t n_pad, int64_t rows, int32_t slices) {
+  if (n_pad <= gpk::NB) return 0;
+  const int64_t h = gpk::trsm_split(n_pad);
+  int64_t need = gpk_gemm_nt_oz_ws_bytes(rows, n_pad - h, h, slices);
+  for (const int64_t part : {gpk_trsm_right_oz_ws_bytes(h, rows, slices), gpk_trsm_right_oz_ws_bytes(n_pad - h, rows, slices)})
+    need = part > need ? part : need;
+  return need;
+}
 int gpk_potrf_f64(double* A, int64_t lda, int64_t a_bstride, int64_t n_pad, int64_t extra_rows, double* logdet,
-                  int32_t* info, int32_t batch, void* stream) {
-  return gpk::potrf_driver<double>(A, lda, a_bstride, n_pad, extra_rows, logdet, info, batch, (cudaStream_t)stream);
+                  int32_t* info, int32_t batch, int32_t slices, void* ws, int64_t ws_bytes, void* stream) {
+  if (const int rc = gpk::oz_check_emulation(slices, ws)) return rc;
+  gpk::Trailing t;
+  // the int8-slice emulation of the trailing updates: one large matrix, and the scratch holds a panel's slices
+  if (slices && batch == 1 && n_pad >= 2048 && ws_bytes >= gpk::oz_ws_bytes(n_pad + extra_rows, gpk::NB_OUTER, slices)) {
+    t.mode = gpk::MODE_OZAKI;
+    t.ws = ws;
+    t.ws_bytes = ws_bytes;
+    t.slices = slices;
+  }
+  return gpk::potrf_driver<double>(A, lda, a_bstride, n_pad, extra_rows, logdet, info, batch, (cudaStream_t)stream, t);
 }
 int gpk_potrf_f64_tf32x3(double* A, int64_t lda, int64_t a_bstride, int64_t n_pad, int64_t extra_rows, double* logdet,
                          int32_t* info, int32_t batch, float* ws, int64_t ws_elems, void* stream) {
@@ -1075,27 +1078,20 @@ int gpk_potrf_f64_tf32x3(double* A, int64_t lda, int64_t a_bstride, int64_t n_pa
   t.ws_bytes = ws_elems * 4;
   return gpk::potrf_driver<double>(A, lda, a_bstride, n_pad, extra_rows, logdet, info, batch, (cudaStream_t)stream, t);
 }
-int gpk_potrf_f64_oz(double* A, int64_t lda, int64_t a_bstride, int64_t n_pad, int64_t extra_rows, double* logdet,
-                     int32_t* info, int32_t batch, int32_t slices, void* ws, int64_t ws_bytes, void* stream) {
-  if (slices < 5 || slices > 8 || !ws || reinterpret_cast<uintptr_t>(ws) % 1024) return GPK_ERR_ARG;
-  gpk::Trailing t;
-  t.mode = gpk::MODE_OZAKI;
-  t.ws = ws;
-  t.ws_bytes = ws_bytes;
-  t.slices = slices;
-  return gpk::potrf_driver<double>(A, lda, a_bstride, n_pad, extra_rows, logdet, info, batch, (cudaStream_t)stream, t);
-}
 int gpk_potrf_f32(float* A, int64_t lda, int64_t a_bstride, int64_t n_pad, int64_t extra_rows, float* logdet,
                   int32_t* info, int32_t batch, void* stream) {
   return gpk::potrf_driver<float>(A, lda, a_bstride, n_pad, extra_rows, logdet, info, batch, (cudaStream_t)stream);
 }
 int gpk_trsm_right_f64(const double* L, int64_t ldl, int64_t l_bstride, int64_t n_pad, double* B, int64_t ldb,
-                       int64_t b_bstride, int64_t rows, int32_t batch, void* stream) {
-  return gpk::trsm_right_driver<double>(L, ldl, l_bstride, n_pad, B, ldb, b_bstride, rows, batch, (cudaStream_t)stream);
+                       int64_t b_bstride, int64_t rows, int32_t batch, int32_t slices, void* ws, int64_t ws_bytes,
+                       void* stream) {
+  return gpk::trsm_right_driver<double>(L, ldl, l_bstride, n_pad, B, ldb, b_bstride, rows, batch, slices, ws, ws_bytes,
+                                        (cudaStream_t)stream);
 }
 int gpk_trsm_right_f32(const float* L, int64_t ldl, int64_t l_bstride, int64_t n_pad, float* B, int64_t ldb,
                        int64_t b_bstride, int64_t rows, int32_t batch, void* stream) {
-  return gpk::trsm_right_driver<float>(L, ldl, l_bstride, n_pad, B, ldb, b_bstride, rows, batch, (cudaStream_t)stream);
+  return gpk::trsm_right_driver<float>(L, ldl, l_bstride, n_pad, B, ldb, b_bstride, rows, batch, 0, nullptr, 0,
+                                       (cudaStream_t)stream);
 }
 int gpk_trsm_right_t_f64(const double* L, int64_t ldl, int64_t l_bstride, int64_t n_pad, double* B, int64_t ldb,
                          int64_t b_bstride, int64_t rows, int32_t batch, void* stream) {

@@ -99,14 +99,16 @@ struct SparseAbi<double> {
                 double* out, int64_t ldo, void* s) {
     return gpk_kernel_matrix_f64(d, x, xg, 0, n, y, yg, 0, n2, dim, 0.0, nullptr, 0, 0.0, GPK_KM_PAD_ZERO, out, ldo, 0, 1, s);
   }
-  static int trsm(const double* L, int64_t ldl, int64_t n, double* B, int64_t ldb, int64_t rows, void* s) {
-    return gpk_trsm_right_f64(L, ldl, 0, n, B, ldb, 0, rows, 1, s);
+  static int trsm(const double* L, int64_t ldl, int64_t n, double* B, int64_t ldb, int64_t rows, int32_t S, void* ws,
+                  int64_t ws_bytes, void* s) {
+    return gpk_trsm_right_f64(L, ldl, 0, n, B, ldb, 0, rows, 1, S, ws, ws_bytes, s);
   }
   static int sq(const double* V, int64_t ldv, int64_t rows, int64_t nc, double* out, void* s) {
     return gpk_row_dot_sq_f64(V, ldv, 0, rows, nc, nullptr, 0, nullptr, out, 0, 1, s);
   }
-  static int syrk(int64_t M, int64_t K, const double* A, int64_t lda, double* C, int64_t ldc, void* s) {
-    return gpk_gemm_nt_f64(M, M, K, 1.0, A, lda, 0, A, lda, 0, 1.0, C, ldc, 0, 1, 1, s);
+  static int syrk(int64_t M, int64_t K, const double* A, int64_t lda, double* C, int64_t ldc, int32_t S, void* ws,
+                  int64_t ws_bytes, void* s) {
+    return gpk_gemm_nt_f64(M, M, K, 1.0, A, lda, 0, A, lda, 0, 1.0, C, ldc, 0, 1, 1, S, ws, ws_bytes, s);
   }
 };
 template <>
@@ -115,13 +117,14 @@ struct SparseAbi<float> {
                 float* out, int64_t ldo, void* s) {
     return gpk_kernel_matrix_f32(d, x, xg, 0, n, y, yg, 0, n2, dim, 0.0, nullptr, 0, 0.0, GPK_KM_PAD_ZERO, out, ldo, 0, 1, s);
   }
-  static int trsm(const float* L, int64_t ldl, int64_t n, float* B, int64_t ldb, int64_t rows, void* s) {
+  static int trsm(const float* L, int64_t ldl, int64_t n, float* B, int64_t ldb, int64_t rows, int32_t, void*, int64_t,
+                  void* s) {
     return gpk_trsm_right_f32(L, ldl, 0, n, B, ldb, 0, rows, 1, s);
   }
   static int sq(const float* V, int64_t ldv, int64_t rows, int64_t nc, float* out, void* s) {
     return gpk_row_dot_sq_f32(V, ldv, 0, rows, nc, nullptr, 0, nullptr, out, 0, 1, s);
   }
-  static int syrk(int64_t M, int64_t K, const float* A, int64_t lda, float* C, int64_t ldc, void* s) {
+  static int syrk(int64_t M, int64_t K, const float* A, int64_t lda, float* C, int64_t ldc, int32_t, void*, int64_t, void* s) {
     return gpk_gemm_nt_f32(M, M, K, 1.0f, A, lda, 0, A, lda, 0, 1.0f, C, ldc, 0, 1, 1, s);
   }
 };
@@ -132,7 +135,8 @@ template <typename T>
 static int sparse_accumulate(const gpk_kernel_desc* desc, const T* xg, int64_t xg_gstride, int64_t c, const T* zg,
                              int64_t zg_gstride, int64_t m, int32_t d, const T* Lz, int64_t ldl, int64_t m_pad,
                              const T* kdiag, const T* kn, const T* ybar, int32_t method, T* A, int64_t lda, T* prod,
-                             T* scalars, T* ws, int64_t ws_elems, void* stream) {
+                             T* scalars, T* ws, int64_t ws_elems, int32_t slices, void* oz_ws, int64_t oz_ws_bytes,
+                             void* stream) {
   if (!desc || !xg || !zg || !Lz || !kn || !ybar || !A || !prod || !scalars || !ws) return GPK_ERR_ARG;
   if (c < 1 || m < 1 || d < 1 || m_pad % 128 || m_pad < m || ldl < m_pad || lda < m_pad) return GPK_ERR_ARG;
   if (method < 0 || method > 2 || (method != 2 && !kdiag)) return GPK_ERR_ARG;
@@ -147,7 +151,7 @@ static int sparse_accumulate(const gpk_kernel_desc* desc, const T* xg, int64_t x
   cudaStream_t s = (cudaStream_t)stream;
   int rc;
   if ((rc = SparseAbi<T>::km(desc, xg, xg_gstride, c, zg, zg_gstride, m, d, Wc, m_pad, stream))) return rc;   // :285
-  if ((rc = SparseAbi<T>::trsm(Lz, ldl, m_pad, Wc, m_pad, c_pad, stream))) return rc;                          // :301
+  if ((rc = SparseAbi<T>::trsm(Lz, ldl, m_pad, Wc, m_pad, c_pad, slices, oz_ws, oz_ws_bytes, stream))) return rc;                          // :301
   if (method != 2 && (rc = SparseAbi<T>::sq(Wc, m_pad, c, m_pad, q, stream))) return rc;                       // :305
   sparse_rows_kernel<T><<<(unsigned)((c_pad + 255) / 256), 256, 0, s>>>(c, c_pad, kdiag, q, kn, ybar, method, rs, ybs, scalars);
   GPK_COUNT_LAUNCH();
@@ -156,7 +160,7 @@ static int sparse_accumulate(const gpk_kernel_desc* desc, const T* xg, int64_t x
   transpose_scaled_kernel<T><<<grid, block, 0, s>>>(Wc, m_pad, c_pad, m_pad, rs, WcT, c_pad);
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();
-  if ((rc = SparseAbi<T>::syrk(m_pad, c_pad, WcT, c_pad, A, lda, stream))) return rc;                           // :322
+  if ((rc = SparseAbi<T>::syrk(m_pad, c_pad, WcT, c_pad, A, lda, slices, oz_ws, oz_ws_bytes, stream))) return rc;                           // :322
   row_dot_acc_kernel<T><<<(unsigned)((m_pad + 7) / 8), 256, 0, s>>>(WcT, c_pad, m_pad, c_pad, ybs, prod);       // :327
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();
@@ -176,15 +180,15 @@ int gpk_sparse_accumulate_f64(const gpk_kernel_desc* desc_host, const double* xg
                               const double* zg, int64_t zg_gstride, int64_t m, int32_t d, const double* Lz, int64_t ldl,
                               int64_t m_pad, const double* kdiag, const double* kn, const double* ybar, int32_t method,
                               double* A, int64_t lda, double* prod, double* scalars, double* ws, int64_t ws_elems,
-                              void* stream) {
+                              int32_t slices, void* oz_ws, int64_t oz_ws_bytes, void* stream) {
   return gpk::sparse_accumulate<double>(desc_host, xg, xg_gstride, c, zg, zg_gstride, m, d, Lz, ldl, m_pad, kdiag, kn, ybar,
-                                        method, A, lda, prod, scalars, ws, ws_elems, stream);
+                                        method, A, lda, prod, scalars, ws, ws_elems, slices, oz_ws, oz_ws_bytes, stream);
 }
 int gpk_sparse_accumulate_f32(const gpk_kernel_desc* desc_host, const float* xg, int64_t xg_gstride, int64_t c,
                               const float* zg, int64_t zg_gstride, int64_t m, int32_t d, const float* Lz, int64_t ldl,
                               int64_t m_pad, const float* kdiag, const float* kn, const float* ybar, int32_t method, float* A,
                               int64_t lda, float* prod, float* scalars, float* ws, int64_t ws_elems, void* stream) {
   return gpk::sparse_accumulate<float>(desc_host, xg, xg_gstride, c, zg, zg_gstride, m, d, Lz, ldl, m_pad, kdiag, kn, ybar,
-                                       method, A, lda, prod, scalars, ws, ws_elems, stream);
+                                       method, A, lda, prod, scalars, ws, ws_elems, 0, nullptr, 0, stream);
 }
 }

@@ -60,7 +60,13 @@ def _require_cuda(*ts):
 
 
 def _fn(name, dtype):
-    return getattr(_lib.load(), f"{name}_{_suffix(dtype)}")
+    """``name_f64`` / ``name_f32`` of libgpk.  An fp64 call that leaves out the emulation arguments ``(slices, ws, ws_bytes)``
+    before the stream runs on the fp64 tensor cores, as with ``(0, NULL, 0)``."""
+    fn = getattr(_lib.load(), f"{name}_{_suffix(dtype)}")
+    if dtype != torch.float64 or "OZ" not in _lib._SIGNATURES.get(name, ()):
+        return fn
+    native = len(fn.argtypes) - 3
+    return lambda *args: fn(*args[:-1], 0, None, 0, args[-1]) if len(args) == native else fn(*args)
 
 
 def launch_count(reset=False):
@@ -205,11 +211,10 @@ def gemm_nt(A, Bm, C=None, *, alpha=1.0, beta=0.0, lower=False):
     for t in (A, Bm, C):
         if t.stride(2) != 1:
             raise ValueError("gemm_nt needs a unit inner stride")
-    if Bn == 1:
-        _emulation_for_gemm(A.device, A.dtype, M, N, K)
+    em = _emulation(A.dtype, A.device, lambda lib, s: lib.gpk_gemm_nt_oz_ws_bytes(M, N, K, s) if Bn == 1 else 0)
     rc = _fn("gpk_gemm_nt", A.dtype)(
         M, N, K, alpha, _ptr(A), A.stride(1), A.stride(0), _ptr(Bm), Bm.stride(1), Bm.stride(0), beta, _ptr(C),
-        C.stride(1), C.stride(0), 1 if lower else 0, Bn, _stream(),
+        C.stride(1), C.stride(0), 1 if lower else 0, Bn, *em, _stream(),
     )
     check(rc, "gpk_gemm_nt")
     return C
@@ -337,12 +342,10 @@ class Chol:
         if Bt.shape[2] != self.n_pad or Bt.shape[1] % TILE or Bt.stride(2) != 1:
             raise ValueError("solve_rows_ needs a padded [B, rows_pad, n_pad] buffer")
         Lp = self.L_padded()
-        if self.batch == 1:  # the recursive solve's largest GEMM: rows x n/2 x n/2
-            h = round_up(self.n_pad // 2)
-            _emulation_for_gemm(self.device, self.dtype, Bt.shape[1], self.n_pad - h + TILE, h)
+        rows, n_pad, batch = Bt.shape[1], self.n_pad, self.batch
+        em = _emulation(self.dtype, self.device, lambda lib, s: lib.gpk_trsm_right_oz_ws_bytes(n_pad, rows, s) if batch == 1 else 0)
         rc = _fn("gpk_trsm_right", self.dtype)(
-            _ptr(Lp), Lp.stride(1), Lp.stride(0), self.n_pad, _ptr(Bt), Bt.stride(1), Bt.stride(0), Bt.shape[1],
-            self.batch, _stream(),
+            _ptr(Lp), Lp.stride(1), Lp.stride(0), n_pad, _ptr(Bt), Bt.stride(1), Bt.stride(0), rows, batch, *em, _stream(),
         )
         check(rc, "gpk_trsm_right")
         return Bt
@@ -428,10 +431,9 @@ def _potrf(W, n, n_pad, extra, k, well_conditioned=False):
                                               B, _ptr(ws), ws.numel(), _stream())
         check(rc, "gpk_potrf_f64_tf32x3")
         return Chol(W, n, k, logdet, info)
-    if W.dtype == torch.float64 and B == 1 and n_pad >= 2048:
-        slices = _oz_slices(well_conditioned)
-        _set_emulation(W.device, slices, _lib.load().gpk_potrf_oz_ws_bytes(n_pad, extra, slices) if slices else 0)
-    rc = _fn("gpk_potrf", W.dtype)(_ptr(W), W.stride(1), W.stride(0), n_pad, extra, _ptr(logdet), _ptr(info), B,
+    em = _emulation(W.dtype, W.device, lambda lib, s: lib.gpk_potrf_oz_ws_bytes(n_pad, extra, s) if B == 1 else 0,
+                    well_conditioned)
+    rc = _fn("gpk_potrf", W.dtype)(_ptr(W), W.stride(1), W.stride(0), n_pad, extra, _ptr(logdet), _ptr(info), B, *em,
                                    _stream())
     check(rc, "gpk_potrf")
     return Chol(W, n, k, logdet, info)
@@ -493,40 +495,27 @@ def _well_conditioned(flat, noise_scalar, noise_vec, jitter):
     return diag >= 1e-3 * max(scale, 1e-300)
 
 
-#: per-device scratch handed to the library for the int8-slice emulation: [tensor, slices registered]
-_EMULATION = {}
-_EMULATION_MAX_BYTES = 8 << 30
+#: per-device scratch of the int8-slice emulation, shared by every call on the device (they are stream-ordered)
+_OZ_SCRATCH = {}
+_OZ_SCRATCH_MAX_BYTES = 8 << 30
 
 
-def _set_emulation(device, slices, need_bytes):
-    """Make the library's fp64 emulation mode on ``device`` match ``B.precision`` and own a scratch buffer of at least
-    ``need_bytes`` (grown on demand, capped: larger requests simply stay on the fp64 tensor cores)."""
-    key = torch.device(device).index or 0
-    buf, cur = _EMULATION.get(key, (None, 0))
-    lib = _lib.load()
-    if slices == 0:
-        if cur:
-            with torch.cuda.device(key):
-                check(lib.gpk_set_f64_emulation(0, None, 0), "gpk_set_f64_emulation")
-            _EMULATION[key] = (buf, 0)
-        return
-    need_bytes = min(int(need_bytes), _EMULATION_MAX_BYTES)
-    if buf is None or buf.numel() < need_bytes:
-        buf = _aligned_bytes(max(need_bytes, 64 << 20), torch.device("cuda", key))
-        cur = 0
-    if cur != slices:
-        with torch.cuda.device(key):
-            check(lib.gpk_set_f64_emulation(slices, _ptr(buf), buf.numel()), "gpk_set_f64_emulation")
-    _EMULATION[key] = (buf, slices)
-
-
-def _emulation_for_gemm(device, dtype, M, N, K):
+def _emulation(dtype, device, need, well_conditioned=False):
+    """The trailing ``(slices, ws, ws_bytes)`` arguments of an fp64 entry point (none for fp32): ``B.precision``'s slice count
+    (:func:`_oz_slices`) and ``device``'s scratch, grown on demand to ``need(lib, slices)`` bytes -- the library's size query
+    for the call -- and capped (larger requests stay on the fp64 tensor cores).  ``(0, NULL, 0)`` when the slice count or
+    the need is 0: the call runs on the fp64 tensor cores."""
     if dtype != torch.float64:
-        return
-    slices = _oz_slices(False)
-    kc = K if K <= 65536 else -(-K // (-(-K // 65536)) // 128) * 128 + 128  # long reductions run in K chunks <= 65536
-    need = _lib.load().gpk_f64_emulation_scratch_bytes(M, N, min(K, kc), slices) if slices and M * N * K >= 1.5e9 else 0
-    _set_emulation(device, slices, need)
+        return ()
+    slices = _oz_slices(well_conditioned)
+    need_bytes = min(int(need(_lib.load(), slices)), _OZ_SCRATCH_MAX_BYTES) if slices else 0
+    if not need_bytes:
+        return 0, None, 0
+    key = torch.device(device).index or 0
+    buf = _OZ_SCRATCH.get(key)
+    if buf is None or buf.numel() < need_bytes:
+        buf = _OZ_SCRATCH[key] = _aligned_bytes(max(need_bytes, 64 << 20), torch.device("cuda", key))
+    return slices, _ptr(buf), buf.numel()
 
 
 def _aligned_bytes(nbytes, device, align=1024):
@@ -610,18 +599,13 @@ def posterior_marginals(flat, xsg, xg, chol, half_y=None, want_sq=True, chunk=40
         return dot, sq
     chunk = min(round_up(chunk), round_up(m))
     ws = torch.empty(chunk * chol.n_pad, dtype=dt, device=dev)
-    if dt == torch.float64:  # the solve's largest product: rows x n/2 x n/2
-        h = round_up(chol.n_pad // 2)
-        slices = _oz_slices(False)
-        need = _lib.load().gpk_f64_emulation_scratch_bytes(chunk, chol.n_pad - h + TILE, h, slices) if (
-            slices and chunk * (chol.n_pad - h + TILE) * h >= 1.5e9) else 0
-        _set_emulation(dev, slices, need)
+    em = _emulation(dt, dev, lambda lib, s: lib.gpk_trsm_right_oz_ws_bytes(chol.n_pad, chunk, s))
     Lp = chol.L_padded()
     hy = None if half_y is None else half_y.contiguous()
     desc = flat.desc()
     rc = _fn("gpk_posterior_marginals", dt)(
         ctypes.byref(desc), _ptr(xsg), xsg.stride(0), m, _ptr(xg), xg.stride(0), xg.shape[2], d, _ptr(Lp), Lp.stride(1),
-        chol.n_pad, _ptr(hy), _ptr(dot), _ptr(sq), chunk, _ptr(ws), ws.numel(), _stream(),
+        chol.n_pad, _ptr(hy), _ptr(dot), _ptr(sq), chunk, _ptr(ws), ws.numel(), *em, _stream(),
     )
     check(rc, "gpk_posterior_marginals")
     return dot, sq
@@ -657,15 +641,6 @@ class SparseAccumulator:
         need = int(self.lib.gpk_sparse_ws_elems(c, self.m_pad))
         if self.ws is None or self.ws.numel() < need:
             self.ws = torch.empty(need, dtype=self.ch.dtype, device=self.ch.device)
-        if self.ch.dtype == torch.float64:
-            # the emulation scratch has to hold the largest product of the solve and the K = c accumulation
-            slices = _oz_slices(False)
-            c_pad, h = round_up(c), round_up(self.m_pad // 2)
-            need_b = 0
-            if slices:
-                f = self.lib.gpk_f64_emulation_scratch_bytes
-                need_b = max(f(self.m_pad, self.m_pad, c_pad, slices), f(c_pad, self.m_pad - h + TILE, h, slices))
-            _set_emulation(self.ch.device, slices, need_b)
         return self.ws
 
     def add(self, xg_chunk, kdiag, kn, ybar):
@@ -676,6 +651,10 @@ class SparseAccumulator:
         if c == 0:
             return
         ws = self._workspace(c)
+        m_pad, c_pad = self.m_pad, round_up(c)
+        # the emulation scratch holds the larger of the solve's products and the K = c accumulation
+        em = _emulation(self.ch.dtype, self.ch.device, lambda lib, s: max(lib.gpk_trsm_right_oz_ws_bytes(m_pad, c_pad, s),
+                                                                          lib.gpk_gemm_nt_oz_ws_bytes(m_pad, m_pad, c_pad, s)))
         kd = None if kdiag is None else kdiag.contiguous()
         kn, ybar = kn.contiguous(), ybar.contiguous()
         Lp = self.ch.L_padded()
@@ -683,7 +662,7 @@ class SparseAccumulator:
         rc = _fn("gpk_sparse_accumulate", self.ch.dtype)(
             ctypes.byref(desc), _ptr(xg_chunk), xg_chunk.stride(0), c, _ptr(self.zg), self.zg.stride(0), self.m, self.d,
             _ptr(Lp), Lp.stride(1), self.m_pad, _ptr(kd), _ptr(kn), _ptr(ybar), self.method, _ptr(self.A), self.A.stride(1),
-            _ptr(self.prod), _ptr(self.scalars), _ptr(ws), ws.numel(), _stream(),
+            _ptr(self.prod), _ptr(self.scalars), _ptr(ws), ws.numel(), *em, _stream(),
         )
         check(rc, "gpk_sparse_accumulate")
 

@@ -12,10 +12,11 @@ epsilon = 1e-12
 #: build, leaf factorisations, panel solves, small problems, batched problems -- always runs in native fp64.
 #:   "auto" (default): fp64 emulated on the int8 tensor cores (wgmma .s32.s8.s8): operands split error-free into signed
 #:       7-bit slices, EXACT int32 slice products, fp64 recombination.  7 slices (49 bits, product error ~3e-14 |a||b|) for
-#:       products that do not feed a factorisation and for factorisations of matrices that are well conditioned by
-#:       construction (known scalar noise >= 1e-6 of the kernel variance): log-pdfs agree with the native path to ~1e-13
-#:       relative -- three orders inside the 1e-10 parity bar, ~2x faster.  8 slices (below) for every other factorisation
-#:       (noise-free kernels on the 1e-12 jitter, posterior covariances, assembled multi-output joints): those can be
+#:       the solve and products of the log-pdf backward and for factorisations of matrices that are well conditioned by
+#:       construction (known scalar noise >= 1e-3 of the kernel variance) inside a log-pdf that is not differentiated:
+#:       log-pdfs agree with the native path to ~1e-13 relative -- three orders inside the 1e-10 parity bar, ~2x faster.
+#:       8 slices (below) for every other factorisation (noise-free kernels on the 1e-12 jitter, posterior covariances,
+#:       assembled multi-output joints, factors a gradient is read from) and every other solve and product: those can be
 #:       numerically singular, where only fp64-grade products keep the pivots positive when native fp64 does.
 #:   "int8x7": 7 slices everywhere the emulation applies.
 #:   "int8x8": 8 slices (56 bits >= the 53 of fp64): product error ~1e-15, the same as the fp64 tensor-core kernel itself.

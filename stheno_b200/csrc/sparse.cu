@@ -14,11 +14,12 @@
 
 namespace gpk {
 
-// per data point of the chunk: corr, method-specific noise, the scale 1/sqrt(K_n'), ybar scaled, and the three ELBO sums
+// per data point of the chunk: corr, method-specific noise, the scale 1/sqrt(K_n'), ybar scaled, and the three ELBO sums of
+// each block of 256 points -> partial[k][blockIdx.x] (reduced by sparse_scalars_kernel: no atomics, so no run-to-run order)
 template <typename T>
 __global__ void sparse_rows_kernel(int64_t c, int64_t c_pad, const T* __restrict__ kdiag, const T* __restrict__ q,
                                    const T* __restrict__ kn, const T* __restrict__ ybar, int32_t method,
-                                   T* __restrict__ rs, T* __restrict__ ybs, T* __restrict__ scalars) {
+                                   T* __restrict__ rs, T* __restrict__ ybs, double* __restrict__ partial) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   double s_log = 0.0, s_yy = 0.0, s_tr = 0.0;
   if (i < c_pad) {
@@ -55,7 +56,28 @@ __global__ void sparse_rows_kernel(int64_t c, int64_t c_pad, const T* __restrict
     double s = 0.0;
 #pragma unroll
     for (int k = 0; k < 8; ++k) s += red[threadIdx.x][k];
-    atomicAdd(scalars + threadIdx.x, (T)s);
+    partial[threadIdx.x * (int64_t)gridDim.x + blockIdx.x] = s;
+  }
+}
+
+// scalars[k] += sum_b partial[k][b] over the nb blocks of sparse_rows_kernel, one block of 256 threads summing in a fixed
+// order: the same chunk adds the same bits on every run
+template <typename T>
+__global__ void sparse_scalars_kernel(const double* __restrict__ partial, int64_t nb, T* __restrict__ scalars) {
+  __shared__ double red[8];
+  for (int k = 0; k < 3; ++k) {
+    double s = 0.0;
+    for (int64_t b = threadIdx.x; b < nb; b += blockDim.x) s += partial[k * nb + b];
+    s = warp_sum(s);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      double t = 0.0;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) t += red[w];
+      scalars[k] += (T)t;
+    }
+    __syncthreads();
   }
 }
 
@@ -65,7 +87,7 @@ __global__ void transpose_scaled_kernel(const T* __restrict__ src, int64_t lds, 
                                         const T* __restrict__ rs, T* __restrict__ dst, int64_t ldd) {
   __shared__ T tile[32][33];
   const int tx = threadIdx.x, ty = threadIdx.y;
-  const int64_t r0 = (int64_t)blockIdx.y * 32, c0 = (int64_t)blockIdx.x * 32;
+  const int64_t r0 = (int64_t)blockIdx.x * 32, c0 = (int64_t)blockIdx.y * 32;  // the long dimension (rows) on grid.x
   for (int i = ty; i < 32; i += 8) {
     const int64_t r = r0 + i, cc = c0 + tx;
     tile[i][tx] = (r < rows && cc < cols) ? src[r * lds + cc] * rs[r] : T(0);
@@ -148,15 +170,20 @@ static int sparse_accumulate(const gpk_kernel_desc* desc, const T* xg, int64_t x
   T* q = WcT + m_pad * c_pad;      // [c_pad]
   T* rs = q + c_pad;
   T* ybs = rs + c_pad;
+  const int64_t nb = (c_pad + 255) / 256;  // blocks of sparse_rows_kernel
+  double* partial = reinterpret_cast<double*>(ybs + c_pad);  // [3][nb]; 8-byte aligned: c_pad is a multiple of 128
   cudaStream_t s = (cudaStream_t)stream;
   int rc;
   if ((rc = SparseAbi<T>::km(desc, xg, xg_gstride, c, zg, zg_gstride, m, d, Wc, m_pad, stream))) return rc;   // :285
   if ((rc = SparseAbi<T>::trsm(Lz, ldl, m_pad, Wc, m_pad, c_pad, slices, oz_ws, oz_ws_bytes, stream))) return rc;                          // :301
   if (method != 2 && (rc = SparseAbi<T>::sq(Wc, m_pad, c, m_pad, q, stream))) return rc;                       // :305
-  sparse_rows_kernel<T><<<(unsigned)((c_pad + 255) / 256), 256, 0, s>>>(c, c_pad, kdiag, q, kn, ybar, method, rs, ybs, scalars);
+  sparse_rows_kernel<T><<<(unsigned)nb, 256, 0, s>>>(c, c_pad, kdiag, q, kn, ybar, method, rs, ybs, partial);
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();
-  dim3 grid((unsigned)(m_pad / 32), (unsigned)(c_pad / 32)), block(32, 8);
+  sparse_scalars_kernel<T><<<1, 256, 0, s>>>(partial, nb, scalars);
+  GPK_COUNT_LAUNCH();
+  GPK_CHECK_LAUNCH();
+  dim3 grid((unsigned)(c_pad / 32), (unsigned)(m_pad / 32)), block(32, 8);
   transpose_scaled_kernel<T><<<grid, block, 0, s>>>(Wc, m_pad, c_pad, m_pad, rs, WcT, c_pad);
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();
@@ -173,7 +200,8 @@ extern "C" {
 
 int64_t gpk_sparse_ws_elems(int64_t c, int64_t m_pad) {
   const int64_t c_pad = gpk::pad128(c);
-  return 2 * c_pad * m_pad + 3 * c_pad;
+  // Wc, WcT, q, rs, ybs, then the per-block ELBO sums: 3 doubles per 256 points (6 elements of either type)
+  return 2 * c_pad * m_pad + 3 * c_pad + 6 * ((c_pad + 255) / 256);
 }
 
 int gpk_sparse_accumulate_f64(const gpk_kernel_desc* desc_host, const double* xg, int64_t xg_gstride, int64_t c,

@@ -104,15 +104,19 @@ __global__ void transpose_kernel(const T* __restrict__ src, int64_t lds, int64_t
   src += (int64_t)blockIdx.z * s_bs;
   dst += (int64_t)blockIdx.z * d_bs;
   const int tx = threadIdx.x, ty = threadIdx.y;
-  const int64_t r0 = (int64_t)blockIdx.y * 32, c0 = (int64_t)blockIdx.x * 32;
-  for (int i = ty; i < 32; i += 8) {
-    const int64_t r = r0 + i, c = c0 + tx;
-    tile[i][tx] = (r < rows && c < cols) ? src[r * lds + c] : T(0);
-  }
-  __syncthreads();
-  for (int i = ty; i < 32; i += 8) {
-    const int64_t r = c0 + i, c = r0 + tx;  // dst is cols x rows
-    if (r < cols && c < rows) dst[r * ldd + c] = tile[tx][i];
+  // row tiles on grid.x (no 65535 limit: rows may be a whole data set); column tiles strided over grid.y
+  const int64_t r0 = (int64_t)blockIdx.x * 32;
+  for (int64_t c0 = (int64_t)blockIdx.y * 32; c0 < cols; c0 += (int64_t)gridDim.y * 32) {
+    for (int i = ty; i < 32; i += 8) {
+      const int64_t r = r0 + i, c = c0 + tx;
+      tile[i][tx] = (r < rows && c < cols) ? src[r * lds + c] : T(0);
+    }
+    __syncthreads();
+    for (int i = ty; i < 32; i += 8) {
+      const int64_t r = c0 + i, c = r0 + tx;  // dst is cols x rows
+      if (r < cols && c < rows) dst[r * ldd + c] = tile[tx][i];
+    }
+    __syncthreads();
   }
 }
 
@@ -184,7 +188,9 @@ __global__ void dmma_probe_kernel(double* out, int iters, double a, double b) {
                           int64_t ldd, int64_t d_bstride, int32_t batch, void* stream) {                               \
     if (!src || !dst || rows < 0 || cols < 0 || batch < 1) return GPK_ERR_ARG;                                         \
     if (rows == 0 || cols == 0) return 0;                                                                              \
-    dim3 grid((unsigned)((cols + 31) / 32), (unsigned)((rows + 31) / 32), (unsigned)batch), block(32, 8);              \
+    const int64_t col_tiles = (cols + 31) / 32;                                                                        \
+    dim3 grid((unsigned)((rows + 31) / 32), (unsigned)(col_tiles < 65535 ? col_tiles : 65535), (unsigned)batch),       \
+        block(32, 8);                                                                                                  \
     gpk::transpose_kernel<T><<<grid, block, 0, (cudaStream_t)stream>>>(src, lds, s_bstride, rows, cols, dst, ldd,      \
                                                                       d_bstride);                                      \
     GPK_COUNT_LAUNCH();                                                                                                \

@@ -285,6 +285,23 @@ int gpk_sparse_accumulate_f32(const gpk_kernel_desc* desc_host, const float* xg,
                               int64_t m_pad, const float* kdiag, const float* kn, const float* ybar, int32_t method, float* A,
                               int64_t lda, float* prod, float* scalars, float* ws, int64_t ws_elems, void* stream);
 
+/* Backward of the streamed ELBO, the per-data-point step of one chunk of `c` points (rows; c_pad = round_up(c), layouts of
+ * gpk_sparse_accumulate).  In: Wc [c_pad x m_pad] (ld ldw) the solved rows w_i^T = k(x_i, z) L_z^-T, U [c_pad x m_pad]
+ * (ld ldu) the rows u_i^T = w_i^T A^-1, s [m_pad] = A^-1 prod (zero padded), q_i = |w_i|^2, kdiag, kn, ybar [c] (q and kdiag
+ * NULL for DTC).  With beta_i = s.w_i, gamma_i = w_i.u_i, kappa_i = kn_i (+ kdiag_i - q_i for FITC), r_i = ybar_i - beta_i,
+ * g_kappa_i = (r_i^2 + gamma_i - kappa_i) / (2 kappa_i^2):
+ *   g_ybar_i = dE/dybar_i = -r_i / kappa_i;   g_kn_i = dE/dkn_i;   g_kd_i = dE/dkdiag_i (not written for DTC);
+ *   row i of U <- g_i^T, g_i = dE/dw_i = (s r_i - u_i) / kappa_i + 2 g_q,i w_i;  rows c .. c_pad - 1 of U are zeroed.
+ *   method 0 (VFE): g_kn = g_kappa + (kdiag - q) / (2 kn^2), g_kd = -1 / (2 kn), g_q = 1 / (2 kn)
+ *   method 1 (FITC): g_kn = g_kd = g_kappa, g_q = -g_kappa;   method 2 (DTC): g_kn = g_kappa, g_q = 0
+ * One warp per row, fp64 accumulation in both precisions, no atomics. */
+int gpk_sparse_rows_bwd_f64(int64_t c, int64_t m_pad, const double* Wc, int64_t ldw, double* U, int64_t ldu, const double* s,
+                            const double* q, const double* kdiag, const double* kn, const double* ybar, int32_t method,
+                            double* g_kn, double* g_kd, double* g_ybar, void* stream);
+int gpk_sparse_rows_bwd_f32(int64_t c, int64_t m_pad, const float* Wc, int64_t ldw, float* U, int64_t ldu, const float* s,
+                            const float* q, const float* kdiag, const float* kn, const float* ybar, int32_t method,
+                            float* g_kn, float* g_kd, float* g_ybar, void* stream);
+
 /* Measurement helper (bench.py): runs a register-resident fp64 tensor-core (DMMA) loop on every SM and returns the
  * achieved TFLOP/s -- the denominator of the fp64 roofline -- or a negative error code.  Synchronises the device. */
 double gpk_probe_dmma_tflops(void);

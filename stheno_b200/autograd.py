@@ -228,6 +228,76 @@ def no_gradient(route, value, inputs):
     return _NoGradient.apply(route, value, *inputs)
 
 
+# ---- the sparse ELBO (PseudoObs VFE / FITC / DTC) -----------------------------------------------------------------------
+#
+# L = chol(K_z + eps I), W = L^-1 K_zx (columns w_i), kappa_i = K_n' (:311-313), A = I + W diag(1/kappa) W^T, s = A^-1 prod.
+# gpk_sparse_rows_bwd gives the per-point gradients and g_i = dE/dw_i; E depends on W only through W^T W, so H = sum_i g_i w_i^T
+# is symmetric and   dE/dK_zx[:, i] = L^-T g_i,   dE/dK_z = -1/2 L^-T H L^-1.
+class SparseElboSpec:
+    """What one sparse ELBO needs beyond its tensor inputs: the method, the flat kernels of ``K_z`` (``flat_z``), of the cross
+    kernel (``flat_c``) and of ``k_x`` (``flat_x``, None for DTC), the chunk, and ``fwd()``, which runs the launches of the
+    no-grad streamed path and returns ``(ch_z, ch_A, s, kdiag, elbo)``."""
+
+    def __init__(self, method, flat_z, flat_c, flat_x, chunk, fwd):
+        self.method, self.flat_z, self.flat_c, self.flat_x, self.chunk, self.fwd = method, flat_z, flat_c, flat_x, chunk, fwd
+
+
+class _SparseElbo(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, spec, coefs_z, zg_z, ns_z, nv_z, coefs_c, xg_c, zg_c, coefs_x, xg_x, kn, ybar):
+        ch_z, ch_A, s, kdiag, elbo = spec.fwd()
+        ctx.spec, ctx.ch_z, ctx.ch_A, ctx.s, ctx.kdiag = spec, ch_z, ch_A, s, kdiag
+        ctx.zg_z, ctx.xg_c, ctx.zg_c = zg_z.detach().contiguous(), xg_c.detach().contiguous(), zg_c.detach().contiguous()
+        ctx.xg_x = None if xg_x is None else xg_x.detach().contiguous()
+        ctx.kn, ctx.ybar = kn.detach(), ybar.detach()
+        ctx.nv_shape = None if nv_z is None else nv_z.shape
+        return elbo
+
+    @staticmethod
+    def backward(ctx, g):
+        spec, ch_z = ctx.spec, ctx.ch_z
+        (_, want_coefs_z, want_zg_z, want_ns, want_nv, want_coefs_c, want_xg_c, want_zg_c, want_coefs_x, want_xg_x, _,
+         _) = ctx.needs_input_grad
+        dt, dev, m = ch_z.dtype, ch_z.device, ch_z.n
+        want_K = want_coefs_z or want_zg_z or want_ns or want_nv
+        ts_c = torch.zeros(1, _lib.GPK_MAX_TERMS, dtype=dt, device=dev) if want_coefs_c else None
+        g_xc = torch.zeros_like(ctx.xg_c) if want_xg_c else None
+        g_zc = torch.zeros_like(ctx.zg_c) if want_zg_c else None
+        g_kn, g_kd, g_y, H = ops.sparse_elbo_bwd(
+            spec.flat_c, ctx.xg_c, ctx.zg_c, ch_z, ctx.ch_A, ctx.s, ctx.kdiag, ctx.kn, ctx.ybar, spec.method, spec.chunk,
+            want_H=want_K, want_cross=want_coefs_c or want_xg_c or want_zg_c, term_sum=ts_c, grad_xg=g_xc, grad_zg=g_zc)
+        grads = dict(kn=g_kn, ybar=g_y, coefs_c=None if ts_c is None else ts_c[0, : len(spec.flat_c.terms)], xg_c=g_xc,
+                     zg_c=g_zc)
+        if want_K:
+            # dE/dK_z = -1/2 L^-T H L^-1: two transposed solves with a transpose between them
+            m_pad = ch_z.n_pad
+            ch_z.solve_many_rows_t_(H)
+            GK = ops.transpose(H, m_pad, m_pad)
+            del H
+            ch_z.solve_many_rows_t_(GK)
+            GK.mul_(-0.5)
+            ops.symmetrize_(GK, m_pad)
+            term_sum, g_zz, diag = _bwd_kernel(spec.flat_z, ctx.zg_z, GK, m)
+            del GK
+            grads.update(coefs_z=term_sum[0, : len(spec.flat_z.terms)] if want_coefs_z else None, zg_z=g_zz if want_zg_z else None,
+                         ns=diag.sum() if want_ns else None, nv=diag.reshape(ctx.nv_shape) if want_nv else None)
+        if want_coefs_x or want_xg_x:
+            fx = spec.flat_x
+            ts_x = torch.zeros(1, _lib.GPK_MAX_TERMS, dtype=dt, device=dev) if want_coefs_x else None
+            g_xx = torch.zeros_like(ctx.xg_x) if want_xg_x else None
+            ops.kernel_cross_bwd(fx, ctx.xg_x, ctx.xg_x, gdiag=g_kd.unsqueeze(0), term_sum=ts_x, grad_xsg=g_xx)
+            grads.update(coefs_x=None if ts_x is None else ts_x[0, : len(fx.terms)], xg_x=g_xx)
+        order = ("coefs_z", "zg_z", "ns", "nv", "coefs_c", "xg_c", "zg_c", "coefs_x", "xg_x", "kn", "ybar")
+        return (None,) + tuple(None if grads.get(k) is None else g * grads[k] for k in order)
+
+
+def sparse_elbo(spec, coefs_z, zg_z, ns_z, nv_z, coefs_c, xg_c, zg_c, coefs_x, xg_x, kn, ybar):
+    """The ELBO ``spec.fwd()`` computes, differentiable w.r.t. the coefficients and pre-stretched inputs of ``K_z``'s kernel
+    (``coefs_z``, ``zg_z``), its scalar and vector noise (``ns_z``, ``nv_z``), the cross kernel's (``coefs_c``, ``xg_c``, ``zg_c``)
+    and ``k_x``'s (``coefs_x``, ``xg_x``; None for DTC), the observation noise ``kn [n]`` and ``ybar [n]``."""
+    return _SparseElbo.apply(spec, coefs_z, zg_z, ns_z, nv_z, coefs_c, xg_c, zg_c, coefs_x, xg_x, kn, ybar)
+
+
 # ---- exact posterior predictions --------------------------------------------------------------------------------------
 #
 # K = k(x, x) + noise + eps I = L L^T,  alpha = K^-1 ybar,  K* = k(x*, x),  V = K* L^-T,  W = V L^-1 = K* K^-1.

@@ -151,6 +151,63 @@ struct SparseAbi<float> {
   }
 };
 
+// Backward of the streamed ELBO, per data point of a chunk (one warp per row; no atomics).  With s = A^-1 prod and the solved
+// rows w_i (Wc) and u_i = A^-1 w_i (U):  beta_i = s.w_i, gamma_i = w_i.u_i, r_i = ybar_i - beta_i, kappa_i = K_n' (:311-313),
+//   g_kappa = (r^2 + gamma - kappa) / (2 kappa^2),  dE/dybar_i = -r / kappa,
+//   dE/dkn_i, dE/dkdiag_i, g_q by method (VFE: g_kappa + (kd - q) / (2 kn^2), -1 / (2 kn), 1 / (2 kn);  FITC: g_kappa, g_kappa,
+//   -g_kappa;  DTC: g_kappa, -, 0),  and row i of U becomes g_i^T = ((-u_i + s r_i) / kappa + 2 g_q w_i)^T = dE/dw_i^T.
+// Rows c .. c_pad - 1 of U are zeroed.  Padding columns of Wc, U and s are zero, so they stay zero.
+template <typename T>
+__global__ void sparse_rows_bwd_kernel(int64_t c, int64_t c_pad, int64_t m_pad, const T* __restrict__ Wc, int64_t ldw,
+                                       T* __restrict__ U, int64_t ldu, const T* __restrict__ s, const T* __restrict__ q,
+                                       const T* __restrict__ kdiag, const T* __restrict__ kn, const T* __restrict__ ybar,
+                                       int32_t method, T* __restrict__ g_kn, T* __restrict__ g_kd, T* __restrict__ g_ybar) {
+  const int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (i >= c_pad) return;
+  const int lane = threadIdx.x & 31;
+  T* u = U + i * ldu;
+  if (i >= c) {
+    for (int64_t j = lane; j < m_pad; j += 32) u[j] = T(0);
+    return;
+  }
+  const T* w = Wc + i * ldw;
+  double beta = 0.0, gamma = 0.0;
+  for (int64_t j = lane; j < m_pad; j += 32) {
+    const double wj = (double)w[j];
+    beta = fma((double)s[j], wj, beta);
+    gamma = fma(wj, (double)u[j], gamma);
+  }
+  beta = warp_sum(beta);
+  gamma = warp_sum(gamma);
+  const double sig = (double)kn[i], yb = (double)ybar[i];
+  double kap = sig, qi = 0.0, kd = 0.0;
+  if (method != 2) {
+    qi = (double)q[i];
+    kd = (double)kdiag[i];
+    if (method == 1) kap += kd - qi;
+  }
+  const double r = yb - beta;
+  const double g_kap = (r * r + gamma - kap) / (2.0 * kap * kap);
+  double g_sig = g_kap, g_q = 0.0;
+  if (method == 0) {
+    g_sig += (kd - qi) / (2.0 * sig * sig);
+    g_q = 0.5 / sig;
+  } else if (method == 1) {
+    g_q = -g_kap;
+  }
+  if (lane == 0) {
+    g_kn[i] = (T)g_sig;
+    g_ybar[i] = (T)(-r / kap);
+    if (method == 0) g_kd[i] = (T)(-0.5 / sig);
+    else if (method == 1) g_kd[i] = (T)g_kap;
+  }
+  const double inv = 1.0 / kap, two_gq = 2.0 * g_q;
+  for (int64_t j = lane; j < m_pad; j += 32) {
+    const double wj = (double)w[j];
+    u[j] = (T)(fma((double)s[j], r, -(double)u[j]) * inv + two_gq * wj);
+  }
+}
+
 static inline int64_t pad128(int64_t v) { return (v + 127) / 128 * 128; }
 
 template <typename T>
@@ -194,9 +251,35 @@ static int sparse_accumulate(const gpk_kernel_desc* desc, const T* xg, int64_t x
   return 0;
 }
 
+template <typename T>
+static int sparse_rows_bwd(int64_t c, int64_t m_pad, const T* Wc, int64_t ldw, T* U, int64_t ldu, const T* s, const T* q,
+                           const T* kdiag, const T* kn, const T* ybar, int32_t method, T* g_kn, T* g_kd, T* g_ybar,
+                           void* stream) {
+  if (!Wc || !U || !s || !kn || !ybar || !g_kn || !g_ybar) return GPK_ERR_ARG;
+  if (c < 1 || m_pad < 128 || m_pad % 128 || ldw < m_pad || ldu < m_pad) return GPK_ERR_ARG;
+  if (method < 0 || method > 2 || (method != 2 && (!q || !kdiag || !g_kd))) return GPK_ERR_ARG;
+  const int64_t c_pad = pad128(c);
+  sparse_rows_bwd_kernel<T><<<(unsigned)(c_pad / 8), 256, 0, (cudaStream_t)stream>>>(c, c_pad, m_pad, Wc, ldw, U, ldu, s, q, kdiag,
+                                                                                    kn, ybar, method, g_kn, g_kd, g_ybar);
+  GPK_COUNT_LAUNCH();
+  GPK_CHECK_LAUNCH();
+  return 0;
+}
+
 }  // namespace gpk
 
 extern "C" {
+
+int gpk_sparse_rows_bwd_f64(int64_t c, int64_t m_pad, const double* Wc, int64_t ldw, double* U, int64_t ldu, const double* s,
+                            const double* q, const double* kdiag, const double* kn, const double* ybar, int32_t method,
+                            double* g_kn, double* g_kd, double* g_ybar, void* stream) {
+  return gpk::sparse_rows_bwd<double>(c, m_pad, Wc, ldw, U, ldu, s, q, kdiag, kn, ybar, method, g_kn, g_kd, g_ybar, stream);
+}
+int gpk_sparse_rows_bwd_f32(int64_t c, int64_t m_pad, const float* Wc, int64_t ldw, float* U, int64_t ldu, const float* s,
+                            const float* q, const float* kdiag, const float* kn, const float* ybar, int32_t method,
+                            float* g_kn, float* g_kd, float* g_ybar, void* stream) {
+  return gpk::sparse_rows_bwd<float>(c, m_pad, Wc, ldw, U, ldu, s, q, kdiag, kn, ybar, method, g_kn, g_kd, g_ybar, stream);
+}
 
 int64_t gpk_sparse_ws_elems(int64_t c, int64_t m_pad) {
   const int64_t c_pad = gpk::pad128(c);

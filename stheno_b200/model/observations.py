@@ -129,6 +129,10 @@ class AbstractPseudoObservations(AbstractObservations):
         return self._get(self._K_z, measure)
 
     def elbo(self, measure):
+        if id(measure) not in self._elbo and self._wants_grad(measure):
+            e = self._elbo_streamed_grad(measure)
+            if e is not None:
+                self._elbo[id(measure)] = e
         e = self._get(self._elbo, measure)
         return from_dev(e, _input_meta(self.fdd.x)[2])
 
@@ -170,7 +174,7 @@ class AbstractPseudoObservations(AbstractObservations):
         if self._wants_grad(measure):
             return self._compute_grad(measure)
         K_z = M.add(pairwise(measure.kernels[p_z], z), noise_z)  # :286
-        self._K_z[id(measure)] = K_z
+        self._K_z.setdefault(id(measure), K_z)
         K_n = noise_x  # :290
         if not isinstance(K_n, M.Diagonal):
             raise RuntimeError(
@@ -186,9 +190,28 @@ class AbstractPseudoObservations(AbstractObservations):
         kn3 = kn.reshape(-1, kn.shape[-1])
         if kn3.shape[0] != ch_z.batch:
             kn3 = kn3.expand(ch_z.batch, -1)
-        streamed = self._stream_plan(measure, ch_z)
+        A, _, sol, elbo, _ = self._elbo_from_factor(measure, ch_z, kn3, yb3)
+        Lz_pad = ch_z.L_lower_()  # strict upper triangle zeroed in place (no copy); identity on the padding
+        solp = torch.zeros(ch_z.batch, ops.TILE, m_pad, dtype=A.dtype, device=A.device)
+        solp[:, :1, :m] = sol
+        mu_rows = ops.gemm_nt(solp, Lz_pad)  # row 0 = (L_z A^-1 prod)^T
+        mu = mean_z + mu_rows[:, 0, :m].reshape(mean_z.shape[:-1]).unsqueeze(-1)  # :329
+        self._mu.setdefault(id(measure), mu)
+        # stored "A" = L_z A L_z^T (:323) as two NT products (A is symmetric)
+        U = ops.gemm_nt(Lz_pad, A)
+        LAL = ops.gemm_nt(U, Lz_pad)
+        self._A.setdefault(id(measure), M.Dense(LAL[:, :m, :m].reshape(K_z.shape), K_z.origin))
+        bs = K_z.shape[:-2]
+        self._elbo.setdefault(id(measure), elbo.reshape(bs) if bs else elbo[0])
+
+    def _elbo_from_factor(self, measure, ch_z, kn3, yb3):
+        """From the factor of ``K_z``: ``A = I + W K_n^-1 W^T`` (symmetric, padded), its factor ``ch_A``, ``sol = A^-1 prod``
+        ``[B, 1, m]``, the ELBO ``[B]`` and, on the streamed route with VFE / FITC, ``diag K_x`` ``[n]`` (else None)."""
+        m, m_pad = ch_z.n, ch_z.n_pad
+        streamed = self._stream_plan(measure, ch_z.batch)
+        kd = None
         if streamed is not None:
-            A, prod, det_kn, yky, trace_part = self._accumulate_streamed(measure, ch_z, kn3, yb3, *streamed)
+            A, prod, det_kn, yky, trace_part, kd = self._accumulate_streamed(measure, ch_z, kn3, yb3, *streamed)
         else:
             A, prod, det_kn, yky, trace_part = self._accumulate_materialised(measure, ch_z, kn3, yb3)
         ops.symmetrize_(A, m_pad)
@@ -196,22 +219,54 @@ class AbstractPseudoObservations(AbstractObservations):
         ch_A = A_mat.chol()
         half = ch_A.half_solve(prod.unsqueeze(1))  # [B, 1, m]  L_A^-1 prod
         sol = ch_A.full_solve(prod.unsqueeze(1))  # A^-1 prod
-        Lz_pad = ch_z.L_lower_()  # strict upper triangle zeroed in place (no copy); identity on the padding
-        solp = torch.zeros(ch_z.batch, ops.TILE, m_pad, dtype=A.dtype, device=A.device)
-        solp[:, :1, :m] = sol
-        mu_rows = ops.gemm_nt(solp, Lz_pad)  # row 0 = (L_z A^-1 prod)^T
-        mu = mean_z + mu_rows[:, 0, :m].reshape(mean_z.shape[:-1]).unsqueeze(-1)  # :329
-        self._mu[id(measure)] = mu
-        # stored "A" = L_z A L_z^T (:323) as two NT products (A is symmetric)
-        U = ops.gemm_nt(Lz_pad, A)
-        LAL = ops.gemm_nt(U, Lz_pad)
-        self._A[id(measure)] = M.Dense(LAL[:, :m, :m].reshape(K_z.shape), K_z.origin)
         # ELBO (:333-336)
         det_part = det_kn + ch_A.logdet
         iqf_part = yky - (half * half).sum((-1, -2))
         elbo = -0.5 * (det_part + iqf_part + trace_part)
-        bs = K_z.shape[:-2]
-        self._elbo[id(measure)] = elbo.reshape(bs) if bs else elbo[0]
+        return A, ch_A, sol, elbo, kd
+
+    # -- analytic streamed gradient (autograd.sparse_elbo): the ELBO under grad of one problem on the GPU ---------------------
+    def _elbo_streamed_grad(self, measure):
+        """The ELBO with the analytic backward of ``autograd.sparse_elbo``, or None when the problem is not covered: it needs
+        the streamed route (:meth:`_stream_plan`), ``k_z`` and ``k_x`` that each flatten to one descriptor, Diagonal noise,
+        Zero or Diagonal inducing noise, and data on a CUDA device."""
+        from ..autograd import SparseElboSpec, coef_tensor, sparse_elbo
+        from ..kernels import Input
+
+        p_x, x, K_n = self.fdd.p, self.fdd.x, self.fdd.noise
+        p_z, z, noise_z = self.u.p, self.u.x, self.u.noise
+        if not isinstance(K_n, M.Diagonal) or not isinstance(noise_z, (M.Zero, M.Diagonal)):
+            return None
+        if not isinstance(x, Input) or not x.t.is_cuda:
+            return None
+        K_z = M.add(pairwise(measure.kernels[p_z], z), noise_z)
+        if not isinstance(K_z, M.KernelDense) or K_z.xg.shape[1] != 1:
+            return None
+        plan = self._stream_plan(measure, 1)
+        if plan is None:
+            return None
+        flat_c, scales_c, _, _ = plan
+        flat_x = coefs_x = xg_x = None
+        if self.method in ("vfe", "fitc"):
+            flat_x, scales_x = measure.kernels[p_x]._flat()
+            if flat_x is None or not flat_x.terms:
+                return None
+            xg_x = x.scaled(scales_x)
+            coefs_x = coef_tensor(flat_x, xg_x)
+        K_z.full_precision = True  # the backward reads L_z^-1 element by element: never the 7-slice factorisation
+        coefs_z, ns_z = K_z.grad_params()
+        xg_c, zg_c = x.scaled(scales_c), z.scaled(scales_c)
+        ybar = (uprank(self.y) - measure.means[p_x].dev(x)).reshape(-1)
+        kn = K_n.diag.reshape(-1)
+
+        def fwd():
+            ch_z = K_z.chol()
+            _, ch_A, sol, elbo, kd = self._elbo_from_factor(measure, ch_z, kn.reshape(1, -1), ybar.reshape(1, -1, 1))
+            return ch_z, ch_A, sol[0, 0], kd, elbo[0]
+
+        spec = SparseElboSpec(self.method, K_z.flat, flat_c, flat_x, B.sparse_chunk, fwd)
+        return sparse_elbo(spec, coefs_z, K_z.xg, ns_z, K_z.noise_vec, coef_tensor(flat_c, xg_c), xg_c, zg_c, coefs_x, xg_x,
+                           kn, ybar)
 
 
     # -- differentiable route (generic_grad.py): used only when something that feeds the ELBO requires grad -----------------
@@ -256,20 +311,20 @@ class AbstractPseudoObservations(AbstractObservations):
         K_z, LAL, mu, elbo = sparse_compute_torch(
             self.method, measure.kernels[p_z], measure.kernels[p_z, p_x], measure.kernels[p_x], z.t, x.t, K_n.diag, nz,
             y_bar, measure.means[p_z].dev(z), B.epsilon)
-        self._K_z[id(measure)] = M.Dense(K_z, z.origin)
-        self._mu[id(measure)] = mu
-        self._A[id(measure)] = M.Dense(LAL, z.origin)
-        self._elbo[id(measure)] = elbo
+        self._K_z.setdefault(id(measure), M.Dense(K_z, z.origin))
+        self._mu.setdefault(id(measure), mu)
+        self._A.setdefault(id(measure), M.Dense(LAL, z.origin))
+        self._elbo.setdefault(id(measure), elbo)
 
 
     # -- the two ways to form A = I + W K_n^-1 W^T, prod = W K_n^-1 ybar and the scalars ------------------------------------
-    def _stream_plan(self, measure, ch_z):
+    def _stream_plan(self, measure, batch):
         """``(flat, scales, x_input, z_input)`` when the problem can be streamed (one problem, numeric inputs, a symmetric
-        cross-kernel that fits one K1 descriptor), else None."""
+        cross-kernel that fits one K1 descriptor), else None.  ``batch``: the number of problems ``K_z`` holds."""
         from ..kernels import Input, _is_multi
 
         p_x, x, p_z, z = self.fdd.p, self.fdd.x, self.u.p, self.u.x
-        if ch_z.batch != 1 or _is_multi(x) or _is_multi(z) or not isinstance(x, Input) or not isinstance(z, Input):
+        if batch != 1 or _is_multi(x) or _is_multi(z) or not isinstance(x, Input) or not isinstance(z, Input):
             return None
         if x.batch_shape or z.batch_shape:
             return None
@@ -282,7 +337,8 @@ class AbstractPseudoObservations(AbstractObservations):
         return flat, scales, x, z
 
     def _accumulate_streamed(self, measure, ch_z, kn3, yb3, flat, scales, x, z):
-        """``gpk_sparse_accumulate`` over chunks of data points: O(chunk m + m^2) device memory."""
+        """``gpk_sparse_accumulate`` over chunks of data points: O(chunk m + m^2) device memory.  Also returns ``diag K_x``
+        (None for DTC)."""
         acc = ops.SparseAccumulator(flat, z.scaled(scales), ch_z, self.method, chunk=B.sparse_chunk)
         xg = x.scaled(scales)  # [G, 1, n, d]
         n = x.n
@@ -294,7 +350,7 @@ class AbstractPseudoObservations(AbstractObservations):
             b_ = min(n, a + acc.chunk)
             acc.add(xg[:, :, a:b_], None if kd is None else kd[a:b_], kn1[a:b_], yb1[a:b_])
         sc = acc.scalars
-        return acc.A, acc.prod[: ch_z.n].unsqueeze(0), sc[0].reshape(1), sc[1].reshape(1), sc[2].reshape(1)
+        return acc.A, acc.prod[: ch_z.n].unsqueeze(0), sc[0].reshape(1), sc[1].reshape(1), sc[2].reshape(1), kd
 
     def _accumulate_materialised(self, measure, ch_z, kn3, yb3):
         """Batched / multi-output / non-flattenable problems: ``W^T = K_xz L_z^-T`` held as one ``[B, n_pad, m_pad]`` buffer."""

@@ -108,14 +108,18 @@ int gpk_kernel_diag_f32(const gpk_kernel_desc* desc_host, const float* xg, int64
 /* K1-backward: contraction of an upstream gradient G = d(loss)/dK (symmetric n x n, ld = ldg) with dK/d(theta) for
  * K = k(x, x) (same points): term_sum[b][t] += sum_ij G_ij prod_f phi_f  (d loss / d coef_t; caller zeroes it; stride
  * GPK_MAX_TERMS), grad_xg[g][b][i][:] = d loss / d x^(g)_i (layout and strides of xg), diag[b][i] = G_ii (noise
- * gradient).  No n x n tensor per hyper-parameter is ever formed.  Replaces torch autograd through
+ * gradient), and, optional (NULL: not formed),
+ *   param_sum[b][f] += sum_ij G_ij coef_t prod_{f' != f in t} phi_f' d phi_f / d fac_param[f]   (stride GPK_MAX_FACTORS;
+ *   caller zeroes it; 0 for kinds without a parameter; GPK_RQ: d loss / d alpha).  No n x n tensor per hyper-parameter is
+ *   ever formed.  Replaces torch autograd through
  * exp / pw_dists2 in the reference's optimisation loop (readme_example13_optimisation_torch.py:46-53). */
 int gpk_kernel_matrix_bwd_f64(const gpk_kernel_desc* desc_host, const double* xg, int64_t xg_gstride,
                               int64_t x_bstride, int64_t n, int32_t d, const double* G, int64_t ldg, int64_t g_bstride,
-                              double* term_sum, double* grad_xg, double* diag, int32_t batch, void* stream);
+                              double* term_sum, double* grad_xg, double* diag, double* param_sum, int32_t batch,
+                              void* stream);
 int gpk_kernel_matrix_bwd_f32(const gpk_kernel_desc* desc_host, const float* xg, int64_t xg_gstride, int64_t x_bstride,
                               int64_t n, int32_t d, const float* G, int64_t ldg, int64_t g_bstride, float* term_sum,
-                              float* grad_xg, float* diag, int32_t batch, void* stream);
+                              float* grad_xg, float* diag, float* param_sum, int32_t batch, void* stream);
 
 /* Rectangular K1-backward: K_ij = k(x*_i, x_j) (m x n) for two DIFFERENT point sets (K1 without GPK_KM_SAME: Delta is
  * [r^2 < 1e-10] with gradient 0, no symmetry factor), upstream gradient given factored:
@@ -126,17 +130,18 @@ int gpk_kernel_matrix_bwd_f32(const gpk_kernel_desc* desc_host, const float* xg,
  *   term_sum[b][t] += sum_ij G_ij prod_f phi_f(i, j) (+ the gdiag term)        -> d loss / d coef_t
  *   grad_xsg[g][b][i][:] += d loss / d x*^(g)_i (layout of xsg)
  *   grad_xg[g][b][j][:] += d loss / d x^(g)_j (layout of xg; chunks of test points add up)
+ *   param_sum[b][f] += as for gpk_kernel_matrix_bwd (the gdiag term adds nothing: RQ's d phi / d alpha is 0 at r = 0)
  * The posterior predictions' backward (autograd.py): G* = g_mu alpha^T - 2 diag(g_var) W with W = K* K^-1. */
 int gpk_kernel_cross_bwd_f64(const gpk_kernel_desc* desc_host, const double* xsg, int64_t xsg_gstride,
                              int64_t xs_bstride, int64_t m, const double* xg, int64_t xg_gstride, int64_t x_bstride,
                              int64_t n, int32_t d, const double* W, int64_t ldw, int64_t w_bstride, const double* r,
                              const double* u, const double* v, const double* gdiag, double* term_sum, double* grad_xsg,
-                             double* grad_xg, int32_t batch, void* stream);
+                             double* grad_xg, double* param_sum, int32_t batch, void* stream);
 int gpk_kernel_cross_bwd_f32(const gpk_kernel_desc* desc_host, const float* xsg, int64_t xsg_gstride, int64_t xs_bstride,
                              int64_t m, const float* xg, int64_t xg_gstride, int64_t x_bstride, int64_t n, int32_t d,
                              const float* W, int64_t ldw, int64_t w_bstride, const float* r, const float* u,
                              const float* v, const float* gdiag, float* term_sum, float* grad_xsg, float* grad_xg,
-                             int32_t batch, void* stream);
+                             float* param_sum, int32_t batch, void* stream);
 
 /* fp64 emulation on the INT8 tensor cores (wgmma .s32.s8.s8; Ozaki splitting): every row of an operand is scaled by a
  * power of two and split error-free into `slices` signed 7-bit integers; the slice products are EXACT in int32 and are

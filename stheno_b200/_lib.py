@@ -40,10 +40,10 @@ _SIGNATURES = {
                           _f64, _i32, _ptr, _i64, _i64, _i32, _ptr],
     "gpk_kernel_diag": [POINTER(KernelDesc), _ptr, _i64, _i64, _ptr, _i64, _i64, _i64, _i32, _i32, _ptr, _i64, _i32,
                         _ptr],
-    "gpk_kernel_matrix_bwd": [POINTER(KernelDesc), _ptr, _i64, _i64, _i64, _i32, _ptr, _i64, _i64, _ptr, _ptr, _ptr, _i32,
-                              _ptr],
+    "gpk_kernel_matrix_bwd": [POINTER(KernelDesc), _ptr, _i64, _i64, _i64, _i32, _ptr, _i64, _i64, _ptr, _ptr, _ptr, _ptr,
+                              _i32, _ptr],
     "gpk_kernel_cross_bwd": [POINTER(KernelDesc), _ptr, _i64, _i64, _i64, _ptr, _i64, _i64, _i64, _i32, _ptr, _i64, _i64,
-                             _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr],
+                             _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr],
     "gpk_gemm_nt": [_i64, _i64, _i64, "T", _ptr, _i64, _i64, _ptr, _i64, _i64, "T", _ptr, _i64, _i64, _i32, _i32, "OZ", _ptr],
     "gpk_potrf": [_ptr, _i64, _i64, _i64, _i64, _ptr, _ptr, _i32, "OZ", _ptr],
     "gpk_trsm_right": [_ptr, _i64, _i64, _i64, _ptr, _i64, _i64, _i64, _i32, "OZ", _ptr],

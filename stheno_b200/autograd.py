@@ -4,7 +4,7 @@ ANALYTIC backward (SURVEY.md section 7 step 8, section 8 row a16):
     d logpdf / dK = 1/2 (alpha alpha^T - K^-1),   alpha = K^-1 (y - mu)
 
 ``K^-1 = L^-T L^-1`` comes from one tensor-core TRSM on the identity and one SYRK; the contraction with ``dK/dtheta``
-(kernel scales, length scales through the pre-stretched inputs, inputs, noise) happens inside the K1-backward kernel
+(kernel scales, length scales through the pre-stretched inputs, inputs, noise, RQ's alpha) happens inside the K1-backward kernel
 (``csrc/kernel_matrix_bwd.cu``) so no ``n x n`` gradient tensor per hyper-parameter is ever formed.  The reference gets
 these gradients from torch autograd through ``exp`` / ``cholesky`` / ``triangular_solve``
 (``readme_example13_optimisation_torch.py:46-53``).
@@ -21,8 +21,10 @@ __all__ = ["kernel_logpdf", "dense_logpdf", "kernel_matrix_grad", "kernel_cross_
            "no_gradient"]
 
 
-def _bwd_kernel(flat, xg, G, n):
-    """``(term_sum [B, T], grad_xg like xg, diag [B, n])`` from the K1-backward kernel."""
+def _bwd_kernel(flat, xg, G, n, param_sum=None):
+    """``(term_sum [B, T], grad_xg like xg, diag [B, n])`` from the K1-backward kernel; with ``param_sum``
+    (``[B, GPK_MAX_FACTORS]``, zeroed by the caller) the same launch also adds the gradient of every factor's shape
+    parameter into it."""
     Bn, d = xg.shape[1], xg.shape[3]
     term_sum = torch.zeros(Bn, _lib.GPK_MAX_TERMS, dtype=xg.dtype, device=xg.device)
     grad_xg = torch.zeros_like(xg)
@@ -30,15 +32,29 @@ def _bwd_kernel(flat, xg, G, n):
     desc = flat.desc()
     rc = ops._fn("gpk_kernel_matrix_bwd", xg.dtype)(
         ctypes.byref(desc), ops._ptr(xg), xg.stride(0), xg.stride(1), n, d, ops._ptr(G), G.stride(1), G.stride(0),
-        ops._ptr(term_sum), ops._ptr(grad_xg), ops._ptr(diag), Bn, ops._stream(),
+        ops._ptr(term_sum), ops._ptr(grad_xg), ops._ptr(diag), ops._ptr(param_sum), Bn, ops._stream(),
     )
     _lib.check(rc, "gpk_kernel_matrix_bwd")
     return term_sum, grad_xg, diag
 
 
+def _param_buf(want, B, like):
+    """A zeroed ``[B, GPK_MAX_FACTORS]`` parameter-gradient output when ``want``, else None."""
+    return torch.zeros(B, _lib.GPK_MAX_FACTORS, dtype=like.dtype, device=like.device) if want else None
+
+
+def _param_grad(flat, param_sum):
+    """The ``[F]`` gradient of :func:`param_tensor` from a ``[B, GPK_MAX_FACTORS]`` parameter sum (None stays None)."""
+    return None if param_sum is None else param_sum[:, : _n_factors(flat)].sum(0)
+
+
+def _n_factors(flat):
+    return sum(len(fs) for _, fs in flat.terms)
+
+
 class _KernelLogpdf(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, coefs, xg, noise_scalar, noise_vec, rhs_t, structure, jitter):
+    def forward(ctx, coefs, xg, noise_scalar, noise_vec, rhs_t, structure, jitter, params):
         # coefs [T], xg [G, B, n, d], noise_scalar [] , noise_vec [B, n] or None, rhs_t [B, k, n]
         flat = ops.FlatKernel([(float(c), fs) for c, fs in zip(coefs.tolist(), structure)], xg.shape[0])
         # the backward reads alpha and K^-1 element by element off this factor: never the 7-slice factorisation
@@ -54,13 +70,14 @@ class _KernelLogpdf(torch.autograd.Function):
     def backward(ctx, g):
         ch, flat, xg = ctx.ch, ctx.flat, ctx.xg
         alpha, Gm = _alpha_and_G(ch, g)
-        term_sum, grad_xg, diag = _bwd_kernel(flat, xg, Gm, ch.n)
+        ps = _param_buf(ctx.needs_input_grad[7], xg.shape[1], xg)
+        term_sum, grad_xg, diag = _bwd_kernel(flat, xg, Gm, ch.n, ps)
         T = len(flat.terms)
         grad_coefs = term_sum[:, :T].sum(0)
         grad_noise_scalar = diag.sum()
         grad_noise_vec = diag if ctx.has_nv else None
         grad_rhs = -g.unsqueeze(-1) * alpha
-        return grad_coefs, grad_xg, grad_noise_scalar, grad_noise_vec, grad_rhs, None, None
+        return grad_coefs, grad_xg, grad_noise_scalar, grad_noise_vec, grad_rhs, None, None, _param_grad(flat, ps)
 
 
 def _alpha_and_G(ch, g):
@@ -123,7 +140,7 @@ class _KernelMatrix(torch.autograd.Function):
     """Differentiable ``k(x, x)`` (same points) built by K1; backward = K1-backward on the symmetrised upstream gradient."""
 
     @staticmethod
-    def forward(ctx, coefs, xg, structure):
+    def forward(ctx, coefs, xg, structure, params):
         flat = ops.FlatKernel([(float(c), fs) for c, fs in zip(coefs.tolist(), structure)], xg.shape[0])
         ctx.flat, ctx.xg = flat, xg.detach().contiguous()
         return ops.kernel_matrix(flat, ctx.xg)
@@ -133,27 +150,44 @@ class _KernelMatrix(torch.autograd.Function):
         flat, xg = ctx.flat, ctx.xg
         n = xg.shape[2]
         Gs = (0.5 * (G + G.transpose(1, 2))).contiguous()  # K is symmetric: only the symmetric part of G matters
-        term_sum, grad_xg, _ = _bwd_kernel(flat, xg, Gs, n)
-        return term_sum[:, : len(flat.terms)].sum(0), grad_xg, None
+        ps = _param_buf(ctx.needs_input_grad[3], xg.shape[1], xg)
+        term_sum, grad_xg, _ = _bwd_kernel(flat, xg, Gs, n, ps)
+        return term_sum[:, : len(flat.terms)].sum(0), grad_xg, None, _param_grad(flat, ps)
+
+
+def _scalar(v, like):
+    """``v`` as a 0-d tensor of ``like``'s dtype and device; a float is converted straight to that dtype (through torch's
+    float32 default it would lose its low bits, and the descriptor built from the tensor with them)."""
+    if isinstance(v, torch.Tensor):
+        return v.to(device=like.device, dtype=like.dtype).reshape(())
+    return torch.tensor(float(v), device=like.device, dtype=like.dtype)
 
 
 def coef_tensor(flat, like):
     """The coefficients of ``flat`` as one ``[T]`` tensor on ``like``'s device, with the graph of those given as tensors."""
     raw = getattr(flat, "coef_raw", None) or [c for c, _ in flat.terms]
-    return torch.stack([
-        (c if isinstance(c, torch.Tensor) else torch.tensor(float(c))).to(device=like.device, dtype=like.dtype).reshape(())
-        for c in raw
-    ])
+    return torch.stack([_scalar(c, like) for c in raw])
+
+
+def param_tensor(flat, like):
+    """The shape parameters of ``flat``'s factors, in descriptor order (RQ's alpha; 0 for kinds without one), as one ``[F]``
+    tensor on ``like``'s device, with the graph of those given as tensors."""
+    vals = [fac[2] if len(fac) > 2 else 0.0 for _, fs in flat.terms for fac in fs]
+    raw = getattr(flat, "param_raw", None) or vals
+    if not vals:
+        return torch.zeros(0, dtype=like.dtype, device=like.device)
+    return torch.stack([_scalar(v if r is None else r, like) for r, v in zip(raw, vals)])
 
 
 def kernel_matrix_grad(flat, xg):
     """``k(x, x) [B, n, n]`` with an autograd graph to the kernel's tensor hyper-parameters and to ``xg``."""
-    return _KernelMatrix.apply(coef_tensor(flat, xg), xg, [fs for _, fs in flat.terms])
+    return _KernelMatrix.apply(coef_tensor(flat, xg), xg, [fs for _, fs in flat.terms], param_tensor(flat, xg))
 
 
-def kernel_logpdf(coefs, xg, noise_scalar, noise_vec, rhs_t, structure, jitter):
-    """Differentiable ``logpdf`` ``[B, k]`` of ``N(0, sum_t coefs[t] prod phi(xg) + noise + jitter I)`` at ``rhs_t``."""
-    return _KernelLogpdf.apply(coefs, xg, noise_scalar, noise_vec, rhs_t, structure, jitter)
+def kernel_logpdf(coefs, xg, noise_scalar, noise_vec, rhs_t, structure, jitter, params=None):
+    """Differentiable ``logpdf`` ``[B, k]`` of ``N(0, sum_t coefs[t] prod phi(xg) + noise + jitter I)`` at ``rhs_t``;
+    ``params``: the factors' shape parameters (:func:`param_tensor`), for their gradient."""
+    return _KernelLogpdf.apply(coefs, xg, noise_scalar, noise_vec, rhs_t, structure, jitter, params)
 
 
 def _flat_of(coefs, structure, n_groups):
@@ -164,7 +198,7 @@ class _KernelCross(torch.autograd.Function):
     """Differentiable ``k(x, y)`` for two different point sets, built by K1; backward = the rectangular K1-backward."""
 
     @staticmethod
-    def forward(ctx, coefs, xsg, xg, structure):
+    def forward(ctx, coefs, xsg, xg, structure, params):
         flat = _flat_of(coefs, structure, xsg.shape[0])
         ctx.flat, ctx.xsg, ctx.xg = flat, xsg.detach().contiguous(), xg.detach().contiguous()
         return ops.kernel_matrix(flat, ctx.xsg, ctx.xg, same=False)
@@ -176,21 +210,22 @@ class _KernelCross(torch.autograd.Function):
         ts = torch.zeros(xsg.shape[1], _lib.GPK_MAX_TERMS, dtype=xsg.dtype, device=xsg.device) if nig[0] else None
         gxs = torch.zeros_like(xsg) if nig[1] else None
         gx = torch.zeros_like(xg) if nig[2] else None
-        ops.kernel_cross_bwd(flat, xsg, xg, W=G.contiguous(), term_sum=ts, grad_xsg=gxs, grad_xg=gx)
-        return None if ts is None else ts[:, : len(flat.terms)].sum(0), gxs, gx, None
+        ps = _param_buf(nig[4], xsg.shape[1], xsg)
+        ops.kernel_cross_bwd(flat, xsg, xg, W=G.contiguous(), term_sum=ts, grad_xsg=gxs, grad_xg=gx, param_sum=ps)
+        return None if ts is None else ts[:, : len(flat.terms)].sum(0), gxs, gx, None, _param_grad(flat, ps)
 
 
 def kernel_cross_grad(flat, xsg, xg):
     """``k(x, y) [B, m, n]`` (``x is not y``) with an autograd graph to the kernel's tensor hyper-parameters, ``xsg`` and
     ``xg``."""
-    return _KernelCross.apply(coef_tensor(flat, xsg), xsg, xg, [fs for _, fs in flat.terms])
+    return _KernelCross.apply(coef_tensor(flat, xsg), xsg, xg, [fs for _, fs in flat.terms], param_tensor(flat, xsg))
 
 
 class _KernelDiag(torch.autograd.Function):
     """Differentiable ``k.elwise(x)`` (same points); the backward is the prior-variance term of the rectangular K1-backward."""
 
     @staticmethod
-    def forward(ctx, coefs, xg, structure):
+    def forward(ctx, coefs, xg, structure, params):
         flat = _flat_of(coefs, structure, xg.shape[0])
         ctx.flat, ctx.xg = flat, xg.detach().contiguous()
         return ops.kernel_diag(flat, ctx.xg)
@@ -201,13 +236,14 @@ class _KernelDiag(torch.autograd.Function):
         nig = ctx.needs_input_grad
         ts = torch.zeros(xg.shape[1], _lib.GPK_MAX_TERMS, dtype=xg.dtype, device=xg.device) if nig[0] else None
         gx = torch.zeros_like(xg) if nig[1] else None
-        ops.kernel_cross_bwd(flat, xg, xg, gdiag=g.contiguous(), term_sum=ts, grad_xsg=gx)
-        return None if ts is None else ts[:, : len(flat.terms)].sum(0), gx, None
+        ps = _param_buf(nig[3], xg.shape[1], xg)
+        ops.kernel_cross_bwd(flat, xg, xg, gdiag=g.contiguous(), term_sum=ts, grad_xsg=gx, param_sum=ps)
+        return None if ts is None else ts[:, : len(flat.terms)].sum(0), gx, None, _param_grad(flat, ps)
 
 
 def kernel_diag_grad(flat, xg):
     """``k.elwise(x) [B, n]`` with an autograd graph to the kernel's tensor hyper-parameters and to ``xg``."""
-    return _KernelDiag.apply(coef_tensor(flat, xg), xg, [fs for _, fs in flat.terms])
+    return _KernelDiag.apply(coef_tensor(flat, xg), xg, [fs for _, fs in flat.terms], param_tensor(flat, xg))
 
 
 class _NoGradient(torch.autograd.Function):
@@ -244,7 +280,8 @@ class SparseElboSpec:
 
 class _SparseElbo(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, spec, coefs_z, zg_z, ns_z, nv_z, coefs_c, xg_c, zg_c, coefs_x, xg_x, kn, ybar):
+    def forward(ctx, spec, coefs_z, zg_z, ns_z, nv_z, coefs_c, xg_c, zg_c, coefs_x, xg_x, kn, ybar, params_z, params_c,
+                params_x):
         ch_z, ch_A, s, kdiag, elbo = spec.fwd()
         ctx.spec, ctx.ch_z, ctx.ch_A, ctx.s, ctx.kdiag = spec, ch_z, ch_A, s, kdiag
         ctx.zg_z, ctx.xg_c, ctx.zg_c = zg_z.detach().contiguous(), xg_c.detach().contiguous(), zg_c.detach().contiguous()
@@ -257,17 +294,19 @@ class _SparseElbo(torch.autograd.Function):
     def backward(ctx, g):
         spec, ch_z = ctx.spec, ctx.ch_z
         (_, want_coefs_z, want_zg_z, want_ns, want_nv, want_coefs_c, want_xg_c, want_zg_c, want_coefs_x, want_xg_x, _,
-         _) = ctx.needs_input_grad
+         _, want_params_z, want_params_c, want_params_x) = ctx.needs_input_grad
         dt, dev, m = ch_z.dtype, ch_z.device, ch_z.n
-        want_K = want_coefs_z or want_zg_z or want_ns or want_nv
+        want_K = want_coefs_z or want_zg_z or want_ns or want_nv or want_params_z
         ts_c = torch.zeros(1, _lib.GPK_MAX_TERMS, dtype=dt, device=dev) if want_coefs_c else None
         g_xc = torch.zeros_like(ctx.xg_c) if want_xg_c else None
         g_zc = torch.zeros_like(ctx.zg_c) if want_zg_c else None
+        ps_c = _param_buf(want_params_c, 1, ctx.xg_c)
         g_kn, g_kd, g_y, H = ops.sparse_elbo_bwd(
             spec.flat_c, ctx.xg_c, ctx.zg_c, ch_z, ctx.ch_A, ctx.s, ctx.kdiag, ctx.kn, ctx.ybar, spec.method, spec.chunk,
-            want_H=want_K, want_cross=want_coefs_c or want_xg_c or want_zg_c, term_sum=ts_c, grad_xg=g_xc, grad_zg=g_zc)
+            want_H=want_K, want_cross=want_coefs_c or want_xg_c or want_zg_c or want_params_c, term_sum=ts_c, grad_xg=g_xc,
+            grad_zg=g_zc, param_sum=ps_c)
         grads = dict(kn=g_kn, ybar=g_y, coefs_c=None if ts_c is None else ts_c[0, : len(spec.flat_c.terms)], xg_c=g_xc,
-                     zg_c=g_zc)
+                     zg_c=g_zc, params_c=_param_grad(spec.flat_c, ps_c))
         if want_K:
             # dE/dK_z = -1/2 L^-T H L^-1: two transposed solves with a transpose between them
             m_pad = ch_z.n_pad
@@ -277,25 +316,32 @@ class _SparseElbo(torch.autograd.Function):
             ch_z.solve_many_rows_t_(GK)
             GK.mul_(-0.5)
             ops.symmetrize_(GK, m_pad)
-            term_sum, g_zz, diag = _bwd_kernel(spec.flat_z, ctx.zg_z, GK, m)
+            ps_z = _param_buf(want_params_z, 1, ctx.zg_z)
+            term_sum, g_zz, diag = _bwd_kernel(spec.flat_z, ctx.zg_z, GK, m, ps_z)
             del GK
             grads.update(coefs_z=term_sum[0, : len(spec.flat_z.terms)] if want_coefs_z else None, zg_z=g_zz if want_zg_z else None,
-                         ns=diag.sum() if want_ns else None, nv=diag.reshape(ctx.nv_shape) if want_nv else None)
-        if want_coefs_x or want_xg_x:
+                         ns=diag.sum() if want_ns else None, nv=diag.reshape(ctx.nv_shape) if want_nv else None,
+                         params_z=_param_grad(spec.flat_z, ps_z))
+        if want_coefs_x or want_xg_x or want_params_x:
             fx = spec.flat_x
             ts_x = torch.zeros(1, _lib.GPK_MAX_TERMS, dtype=dt, device=dev) if want_coefs_x else None
             g_xx = torch.zeros_like(ctx.xg_x) if want_xg_x else None
-            ops.kernel_cross_bwd(fx, ctx.xg_x, ctx.xg_x, gdiag=g_kd.unsqueeze(0), term_sum=ts_x, grad_xsg=g_xx)
-            grads.update(coefs_x=None if ts_x is None else ts_x[0, : len(fx.terms)], xg_x=g_xx)
-        order = ("coefs_z", "zg_z", "ns", "nv", "coefs_c", "xg_c", "zg_c", "coefs_x", "xg_x", "kn", "ybar")
+            ps_x = _param_buf(want_params_x, 1, ctx.xg_x)
+            ops.kernel_cross_bwd(fx, ctx.xg_x, ctx.xg_x, gdiag=g_kd.unsqueeze(0), term_sum=ts_x, grad_xsg=g_xx, param_sum=ps_x)
+            grads.update(coefs_x=None if ts_x is None else ts_x[0, : len(fx.terms)], xg_x=g_xx, params_x=_param_grad(fx, ps_x))
+        order = ("coefs_z", "zg_z", "ns", "nv", "coefs_c", "xg_c", "zg_c", "coefs_x", "xg_x", "kn", "ybar", "params_z",
+                 "params_c", "params_x")
         return (None,) + tuple(None if grads.get(k) is None else g * grads[k] for k in order)
 
 
-def sparse_elbo(spec, coefs_z, zg_z, ns_z, nv_z, coefs_c, xg_c, zg_c, coefs_x, xg_x, kn, ybar):
+def sparse_elbo(spec, coefs_z, zg_z, ns_z, nv_z, coefs_c, xg_c, zg_c, coefs_x, xg_x, kn, ybar, params_z=None, params_c=None,
+                params_x=None):
     """The ELBO ``spec.fwd()`` computes, differentiable w.r.t. the coefficients and pre-stretched inputs of ``K_z``'s kernel
     (``coefs_z``, ``zg_z``), its scalar and vector noise (``ns_z``, ``nv_z``), the cross kernel's (``coefs_c``, ``xg_c``, ``zg_c``)
-    and ``k_x``'s (``coefs_x``, ``xg_x``; None for DTC), the observation noise ``kn [n]`` and ``ybar [n]``."""
-    return _SparseElbo.apply(spec, coefs_z, zg_z, ns_z, nv_z, coefs_c, xg_c, zg_c, coefs_x, xg_x, kn, ybar)
+    and ``k_x``'s (``coefs_x``, ``xg_x``; None for DTC), the observation noise ``kn [n]``, ``ybar [n]`` and the three kernels'
+    shape parameters (``params_z``, ``params_c``, ``params_x``: :func:`param_tensor`)."""
+    return _SparseElbo.apply(spec, coefs_z, zg_z, ns_z, nv_z, coefs_c, xg_c, zg_c, coefs_x, xg_x, kn, ybar, params_z, params_c,
+                             params_x)
 
 
 # ---- exact posterior predictions --------------------------------------------------------------------------------------
@@ -317,7 +363,7 @@ class PosteriorSpec:
 
 class _ExactPosterior(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, spec, coefs_x, xg_x, noise_s, noise_v, ybar, coefs_c, xsg, zg, P):
+    def forward(ctx, spec, coefs_x, xg_x, noise_s, noise_v, ybar, coefs_c, xsg, zg, P, params_x, params_c):
         ctx.set_materialize_grads(False)
         ctx.spec = spec
         ctx.xg_x, ctx.xsg, ctx.zg = xg_x.detach().contiguous(), xsg.detach().contiguous(), zg.detach().contiguous()
@@ -336,23 +382,25 @@ class _ExactPosterior(torch.autograd.Function):
         return (None,) + _posterior_backward(ctx, g_dot, g_sq, g_cov)
 
 
-def exact_posterior(spec, coefs_x, xg_x, noise_s, noise_v, ybar, coefs_c, xsg, zg, P=None):
+def exact_posterior(spec, coefs_x, xg_x, noise_s, noise_v, ybar, coefs_c, xsg, zg, P=None, params_x=None, params_c=None):
     """``(dot, sq, cov)`` of the exact posterior as ``spec.fwd()`` computes them (an empty tensor for those not formed),
     differentiable w.r.t. ``K_x``'s coefficients, inputs ``xg_x`` and noise, ``ybar [B, n]``, the cross kernel's coefficients,
-    the test points ``xsg``, the data points ``zg`` (both stretched by the cross kernel's length scales) and the prior
-    covariance ``P`` of ``cov``."""
-    return _ExactPosterior.apply(spec, coefs_x, xg_x, noise_s, noise_v, ybar, coefs_c, xsg, zg, P)
+    the test points ``xsg``, the data points ``zg`` (both stretched by the cross kernel's length scales), the prior
+    covariance ``P`` of ``cov`` and the shape parameters of ``K_x``'s and the cross kernel (``params_x``, ``params_c``:
+    :func:`param_tensor`)."""
+    return _ExactPosterior.apply(spec, coefs_x, xg_x, noise_s, noise_v, ybar, coefs_c, xsg, zg, P, params_x, params_c)
 
 
 def _posterior_backward(ctx, a, s, gc):
     spec, ch = ctx.spec, ctx.spec.ch
     flat_c, flat_x = spec.flat_c, spec.flat_x
     xsg, zg, xg_x = ctx.xsg, ctx.zg, ctx.xg_x
-    _, want_coefs_x, want_xg_x, want_ns, want_nv, want_y, want_coefs_c, want_xs, want_z, want_P = ctx.needs_input_grad
+    (_, want_coefs_x, want_xg_x, want_ns, want_nv, want_y, want_coefs_c, want_xs, want_z, want_P, want_params_x,
+     want_params_c) = ctx.needs_input_grad
     Bn, n, n_pad, m = ch.batch, ch.n, ch.n_pad, xsg.shape[2]
     dt, dev = ch.dtype, ch.device
-    want_K = want_coefs_x or want_xg_x or want_ns or want_nv
-    want_cross = want_coefs_c or want_xs or want_z
+    want_K = want_coefs_x or want_xg_x or want_ns or want_nv or want_params_x
+    want_cross = want_coefs_c or want_xs or want_z or want_params_c
     a = None if a is None else a.reshape(Bn, m)
     s = None if s is None else s.reshape(Bn, m)
     need_W = (s is not None or gc is not None) and (want_cross or want_K)
@@ -373,7 +421,8 @@ def _posterior_backward(ctx, a, s, gc):
     g_xs = torch.zeros_like(xsg) if want_xs else None
     g_z = torch.zeros_like(zg) if want_z else None
     GK = torch.zeros(Bn, n_pad, n_pad, dtype=dt, device=dev) if want_K else None
-    cross_out = dict(term_sum=ts_c, grad_xg=g_z)
+    ps_c = _param_buf(want_params_c, Bn, xsg)
+    cross_out = dict(term_sum=ts_c, grad_xg=g_z, param_sum=ps_c)
     fac = dict(u=a, v=alpha) if a is not None else {}
 
     if not need_W:
@@ -416,7 +465,7 @@ def _posterior_backward(ctx, a, s, gc):
             Yt = ops.transpose(Y, mp, n_pad)
             ops.gemm_nt(Wt, Yt, GK, alpha=-0.5, beta=1.0, lower=True)
 
-    grad_coefs_x = grad_xg_x = grad_ns = grad_nv = None
+    grad_coefs_x = grad_xg_x = grad_ns = grad_nv = grad_params_x = None
     if want_K:
         if a is not None:  # GK -= (beta alpha^T + alpha beta^T) / 2
             A2 = torch.zeros(Bn, n_pad, 16, dtype=dt, device=dev)
@@ -425,8 +474,10 @@ def _posterior_backward(ctx, a, s, gc):
             B2[:, :n, 0], B2[:, :n, 1] = alpha, beta
             ops.gemm_nt(A2, B2, GK, alpha=-0.5, beta=1.0, lower=True)
         ops.symmetrize_(GK, n_pad)
-        term_sum, grad_xg_x, diag = _bwd_kernel(flat_x, xg_x, GK, n)
+        ps_x = _param_buf(want_params_x, Bn, xg_x)
+        term_sum, grad_xg_x, diag = _bwd_kernel(flat_x, xg_x, GK, n, ps_x)
         del GK
+        grad_params_x = _param_grad(flat_x, ps_x)
         grad_coefs_x = term_sum[:, : len(flat_x.terms)].sum(0) if want_coefs_x else None
         grad_xg_x = grad_xg_x if want_xg_x else None
         grad_ns = diag.sum() if want_ns else None
@@ -438,7 +489,8 @@ def _posterior_backward(ctx, a, s, gc):
         g = gc.reshape(-1, m, m)
         grad_P = (torch.tril(g + g.transpose(1, 2), -1) + torch.diag_embed(torch.diagonal(g, dim1=1, dim2=2)))
         grad_P = grad_P.reshape(ctx.P_shape)
-    return grad_coefs_x, grad_xg_x, grad_ns, grad_nv, grad_y, grad_coefs_c, g_xs, g_z, grad_P
+    return (grad_coefs_x, grad_xg_x, grad_ns, grad_nv, grad_y, grad_coefs_c, g_xs, g_z, grad_P, grad_params_x,
+            _param_grad(flat_c, ps_c))
 
 
 def _solved_rows(ch, flat_c, xs_c, zg):

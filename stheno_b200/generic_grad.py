@@ -25,7 +25,8 @@ def _t(v, like):
 
 
 def kernel_needs_grad(k):
-    """True if a coefficient or length scale of the (flattenable) kernel expression ``k`` is a tensor that requires grad."""
+    """True if a coefficient, length scale or shape parameter (RQ's alpha) of the (flattenable) kernel expression ``k`` is a
+    tensor that requires grad."""
     terms = k.flat_terms() if k is not None else None
     if not terms:
         return False
@@ -33,9 +34,9 @@ def kernel_needs_grad(k):
         if isinstance(coef, torch.Tensor) and coef.requires_grad:
             return True
         for f in fs:
-            s = f[1]
-            if isinstance(s, torch.Tensor) and s.requires_grad:
-                return True
+            for s in f[1:3]:
+                if isinstance(s, torch.Tensor) and s.requires_grad:
+                    return True
     return False
 
 

@@ -229,7 +229,7 @@ class Kernel:
         if terms is None:
             return None, None
         scales, keys = [], {}
-        out, raw = [], []
+        out, raw, praw = [], [], []
         for coef, fs in terms:
             nf = []
             for fac in fs:  # (kind, scale) or (kind, scale, shape parameter)
@@ -238,8 +238,9 @@ class Kernel:
                 if k not in keys:
                     keys[k] = len(scales)
                     scales.append(s)
-                nf.append((kind, keys[k]) + tuple(fac[2:3]))
-            out.append((float(coef.detach()) if isinstance(coef, torch.Tensor) else float(coef), nf))
+                nf.append((kind, keys[k]) + tuple(_value(v) for v in fac[2:3]))
+                praw.append(fac[2] if len(fac) > 2 else None)
+            out.append((_value(coef), nf))
             raw.append(coef)
         if not scales:
             scales = [None]
@@ -249,8 +250,10 @@ class Kernel:
             # more product terms / factors / length scales than one K1 descriptor holds: not flattenable as a whole; the
             # callers fall back to evaluating the children separately (each child gets its own descriptor) and combining
             return None, None
-        # hyper-parameters given as torch tensors that require grad: remember them for the differentiable path
-        flat.coef_raw = raw if any(isinstance(c, torch.Tensor) and c.requires_grad for c in raw) else None
+        # hyper-parameters given as torch tensors that require grad: remember them for the differentiable path (coef_raw
+        # per term, param_raw per factor: the shape parameters, RQ's alpha)
+        flat.coef_raw = raw if any(_requires_grad(c) for c in raw) else None
+        flat.param_raw = praw if any(_requires_grad(v) for v in praw) else None
         return flat, scales
 
     def _flattenable(self):
@@ -266,7 +269,7 @@ class Kernel:
             return torch.zeros(x.batch_shape + (x.n, y.n), dtype=x.t.dtype, device=x.t.device)
         xg = x.scaled(scales)
         yg = xg if same else y.scaled(scales)
-        if torch.is_grad_enabled() and (flat.coef_raw is not None or xg.requires_grad or yg.requires_grad):
+        if torch.is_grad_enabled() and (_flat_needs_grad(flat) or xg.requires_grad or yg.requires_grad):
             from .autograd import kernel_cross_grad, kernel_matrix_grad
 
             K = kernel_matrix_grad(flat, xg) if same else kernel_cross_grad(flat, xg, yg)
@@ -282,7 +285,7 @@ class Kernel:
             return torch.zeros(x.batch_shape + (x.n, 1), dtype=x.t.dtype, device=x.t.device)
         xg = x.scaled(scales)
         yg = xg if same else y.scaled(scales)
-        if torch.is_grad_enabled() and (flat.coef_raw is not None or xg.requires_grad or yg.requires_grad):
+        if torch.is_grad_enabled() and (_flat_needs_grad(flat) or xg.requires_grad or yg.requires_grad):
             from .autograd import kernel_diag_grad, no_gradient
 
             if same:
@@ -315,6 +318,20 @@ class Kernel:
     @property
     def stationary(self):
         return False
+
+
+def _value(v):
+    """A hyper-parameter as a float for the K1 descriptor (a tensor is detached first: no graph, no warning)."""
+    return float(v.detach()) if isinstance(v, torch.Tensor) else float(v)
+
+
+def _requires_grad(v):
+    return isinstance(v, torch.Tensor) and v.requires_grad
+
+
+def _flat_needs_grad(flat):
+    """True if a coefficient or shape parameter of the flat kernel was given as a tensor that requires grad."""
+    return getattr(flat, "coef_raw", None) is not None or getattr(flat, "param_raw", None) is not None
 
 
 def _as_kernel(k):
@@ -358,13 +375,23 @@ class Matern52(_Elementary):
 
 
 class RQ(_Elementary):
-    """Rational quadratic ``(1 + r^2 / (2 alpha))^-alpha`` (mlkernels ``RQ(alpha)``; ``README.md:1076-1088``)."""
+    """Rational quadratic ``(1 + r^2 / (2 alpha))^-alpha`` (mlkernels ``RQ(alpha)``; ``README.md:1076-1088``).  ``alpha``: a
+    number, a NumPy scalar or a one-element torch tensor; a tensor that requires grad receives its gradient on every route
+    with an analytic backward."""
 
     kind = "rq"
 
     def __init__(self, alpha):
-        self.alpha = float(alpha)
-        if not self.alpha > 0:
+        if isinstance(alpha, torch.Tensor):
+            if alpha.numel() != 1:
+                raise ValueError(f"RQ takes one alpha, not a tensor of shape {tuple(alpha.shape)}")
+            self.alpha = alpha if alpha.dim() == 0 else alpha.reshape(())
+        else:
+            a = np.asarray(alpha, np.float64)
+            if a.size != 1:
+                raise ValueError(f"RQ takes one alpha, not an array of shape {a.shape}")
+            self.alpha = float(a.reshape(()))
+        if not _value(self.alpha) > 0:
             raise ValueError("RQ needs alpha > 0")
 
     def flat_terms(self):
@@ -950,7 +977,7 @@ def _grad_tensors(*objs):
         elif isinstance(o, FDD):
             walk(o.x)
         elif isinstance(o, M.KernelDense):
-            walk([getattr(o.flat, "coef_raw", None), o.xg, o.noise_t, o.noise_vec])
+            walk([getattr(o.flat, "coef_raw", None), getattr(o.flat, "param_raw", None), o.xg, o.noise_t, o.noise_vec])
         elif isinstance(o, (Kernel, Mean, InputMap, M.AbstractMatrix)):
             for k, v in vars(o).items():
                 if k not in ("_chol", "_b"):
@@ -978,19 +1005,20 @@ def _exact_route(K_z, k_zi, z, x, *others):
     xsg, zg = xi.scaled(scales), zi.scaled(scales)
     if xsg.shape[1] != K_z.xg.shape[1] or zg.shape[1] != K_z.xg.shape[1] or zg.shape[2] != K_z.n:
         return None, ts
-    from .autograd import coef_tensor
+    from .autograd import coef_tensor, param_tensor
 
     coefs_x, ns = K_z.grad_params()
-    return (flat, [coefs_x, K_z.xg, ns, K_z.noise_vec, coef_tensor(flat, xsg), xsg, zg]), ts
+    return (flat, [coefs_x, K_z.xg, ns, K_z.noise_vec, coef_tensor(flat, xsg), xsg, zg, param_tensor(K_z.flat, K_z.xg),
+                   param_tensor(flat, xsg)]), ts
 
 
 def _exact_posterior(K_z, route, ybar, fwd, half_y=None, P=None):
     """``(dot, sq, cov)`` from ``fwd()`` with the analytic backward of ``autograd.exact_posterior``."""
     from .autograd import PosteriorSpec, exact_posterior
 
-    flat, (coefs_x, xg_x, ns, nv, coefs_c, xsg, zg) = route
+    flat, (coefs_x, xg_x, ns, nv, coefs_c, xsg, zg, params_x, params_c) = route
     spec = PosteriorSpec(K_z.chol(), K_z.flat, flat, half_y, fwd)
-    return exact_posterior(spec, coefs_x, xg_x, ns, nv, ybar, coefs_c, xsg, zg, P)
+    return exact_posterior(spec, coefs_x, xg_x, ns, nv, ybar, coefs_c, xsg, zg, P, params_x, params_c)
 
 
 def _uncovered(route, value, ts):

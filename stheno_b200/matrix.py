@@ -199,6 +199,7 @@ class KernelDense(Dense):
     def needs_grad(self):
         return torch.is_grad_enabled() and (
             getattr(self.flat, "coef_raw", None) is not None
+            or getattr(self.flat, "param_raw", None) is not None
             or self.xg.requires_grad
             or (self.noise_t is not None and self.noise_t.requires_grad)
             or (self.noise_vec is not None and self.noise_vec.requires_grad)
@@ -225,13 +226,14 @@ class KernelDense(Dense):
                                     jitter=_B.epsilon, rhs_t=rhs_t, full_precision=self.full_precision)
 
     def logpdf_grad(self, rhs_t):
-        """Differentiable ``logpdf`` ``[B, k]`` w.r.t. kernel scales, length scales / inputs (through ``xg``), noise and
-        the right-hand sides."""
-        from .autograd import kernel_logpdf
+        """Differentiable ``logpdf`` ``[B, k]`` w.r.t. kernel scales, length scales / inputs (through ``xg``), shape
+        parameters (RQ's alpha), noise and the right-hand sides."""
+        from .autograd import kernel_logpdf, param_tensor
 
         coefs, ns = self.grad_params()
         structure = [fs for _, fs in self.flat.terms]
-        return kernel_logpdf(coefs, self.xg, ns, self.noise_vec, rhs_t, structure, _B.epsilon)
+        return kernel_logpdf(coefs, self.xg, ns, self.noise_vec, rhs_t, structure, _B.epsilon,
+                             param_tensor(self.flat, self.xg))
 
     def grad_params(self):
         """``(coefs [T], scalar noise [])`` as tensors carrying the graph of those given as tensors that require grad."""

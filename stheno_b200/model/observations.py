@@ -230,7 +230,7 @@ class AbstractPseudoObservations(AbstractObservations):
         """The ELBO with the analytic backward of ``autograd.sparse_elbo``, or None when the problem is not covered: it needs
         the streamed route (:meth:`_stream_plan`), ``k_z`` and ``k_x`` that each flatten to one descriptor, Diagonal noise,
         Zero or Diagonal inducing noise, and data on a CUDA device."""
-        from ..autograd import SparseElboSpec, coef_tensor, sparse_elbo
+        from ..autograd import SparseElboSpec, coef_tensor, param_tensor, sparse_elbo
         from ..kernels import Input
 
         p_x, x, K_n = self.fdd.p, self.fdd.x, self.fdd.noise
@@ -246,13 +246,13 @@ class AbstractPseudoObservations(AbstractObservations):
         if plan is None:
             return None
         flat_c, scales_c, _, _ = plan
-        flat_x = coefs_x = xg_x = None
+        flat_x = coefs_x = xg_x = params_x = None
         if self.method in ("vfe", "fitc"):
             flat_x, scales_x = measure.kernels[p_x]._flat()
             if flat_x is None or not flat_x.terms:
                 return None
             xg_x = x.scaled(scales_x)
-            coefs_x = coef_tensor(flat_x, xg_x)
+            coefs_x, params_x = coef_tensor(flat_x, xg_x), param_tensor(flat_x, xg_x)
         K_z.full_precision = True  # the backward reads L_z^-1 element by element: never the 7-slice factorisation
         coefs_z, ns_z = K_z.grad_params()
         xg_c, zg_c = x.scaled(scales_c), z.scaled(scales_c)
@@ -266,7 +266,7 @@ class AbstractPseudoObservations(AbstractObservations):
 
         spec = SparseElboSpec(self.method, K_z.flat, flat_c, flat_x, B.sparse_chunk, fwd)
         return sparse_elbo(spec, coefs_z, K_z.xg, ns_z, K_z.noise_vec, coef_tensor(flat_c, xg_c), xg_c, zg_c, coefs_x, xg_x,
-                           kn, ybar)
+                           kn, ybar, param_tensor(K_z.flat, K_z.xg), param_tensor(flat_c, xg_c), params_x)
 
 
     # -- differentiable route (generic_grad.py): used only when something that feeds the ELBO requires grad -----------------

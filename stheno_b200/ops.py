@@ -173,14 +173,15 @@ def kernel_diag(flat, xg, yg=None, *, same=None):
 
 
 def kernel_cross_bwd(flat, xsg, xg, *, W=None, r=None, u=None, v=None, gdiag=None, term_sum=None, grad_xsg=None,
-                     grad_xg=None):
+                     grad_xg=None, param_sum=None):
     """Rectangular K1-backward (``gpk_kernel_cross_bwd``) of ``K = k(x*, x)`` ``[B, m, n]`` for the upstream gradient
     ``G_ij = r_i W_ij + u_i v_j`` (+ ``gdiag_i`` on ``k(x*_i, x*_i)``).  ``W``: ``[B, >= m, ldw]`` with a unit inner stride;
     ``r``, ``u``, ``gdiag``: ``[B, m]``; ``v``: ``[B, n]``.  The outputs ``term_sum [B, GPK_MAX_TERMS]``, ``grad_xsg`` (like
-    ``xsg``) and ``grad_xg`` (like ``xg``) are accumulated into; pass the ones wanted (None: not formed)."""
+    ``xsg``), ``grad_xg`` (like ``xg``) and ``param_sum [B, GPK_MAX_FACTORS]`` (the gradient of every factor's shape
+    parameter, RQ's alpha) are accumulated into; pass the ones wanted (None: not formed)."""
     _check_groups(xsg, flat)
     _check_groups(xg, flat)
-    _require_cuda(xsg, xg, W, r, u, v, gdiag, term_sum, grad_xsg, grad_xg)
+    _require_cuda(xsg, xg, W, r, u, v, gdiag, term_sum, grad_xsg, grad_xg, param_sum)
     for t, like in ((grad_xsg, xsg), (grad_xg, xg)):
         if t is not None and (t.shape != like.shape or not t.is_contiguous()):
             raise ValueError("kernel_cross_bwd: gradient outputs must be contiguous and shaped like their inputs")
@@ -194,7 +195,7 @@ def kernel_cross_bwd(flat, xsg, xg, *, W=None, r=None, u=None, v=None, gdiag=Non
     rc = _fn("gpk_kernel_cross_bwd", xsg.dtype)(
         ctypes.byref(desc), _ptr(xsg), xsg.stride(0), xsg.stride(1), m, _ptr(xg), xg.stride(0), xg.stride(1), n, d,
         _ptr(W), (W.stride(1) if W is not None else 0), (W.stride(0) if W is not None else 0), _ptr(r), _ptr(u), _ptr(v),
-        _ptr(gdiag), _ptr(term_sum), _ptr(grad_xsg), _ptr(grad_xg), B, _stream(),
+        _ptr(gdiag), _ptr(term_sum), _ptr(grad_xsg), _ptr(grad_xg), _ptr(param_sum), B, _stream(),
     )
     check(rc, "gpk_kernel_cross_bwd")
 
@@ -670,7 +671,7 @@ class SparseAccumulator:
 
 
 def sparse_elbo_bwd(flat, xg, zg, ch_z, ch_A, s, kdiag, kn, ybar, method, chunk, want_H=True, want_cross=True,
-                    term_sum=None, grad_xg=None, grad_zg=None):
+                    term_sum=None, grad_xg=None, grad_zg=None, param_sum=None):
     """Backward of the ELBO :class:`SparseAccumulator` streams, over the same chunks of data points.  ``flat``, ``xg [G, 1, n, d]``,
     ``zg [G, 1, m, d]``: the cross kernel and its pre-stretched inputs; ``ch_z``: factor of ``K_z``; ``ch_A``: factor of
     ``A = I + W K_n^-1 W^T``; ``s = A^-1 prod [m]``; ``kdiag`` (None for DTC), ``kn``, ``ybar``: ``[n]``.
@@ -678,10 +679,10 @@ def sparse_elbo_bwd(flat, xg, zg, ch_z, ch_A, s, kdiag, kn, ybar, method, chunk,
     Per chunk: K1 rows and the solve give ``W_c`` (the forward's launches), ``U_c = W_c A^-1``, and ``gpk_sparse_rows_bwd`` turns
     ``U_c`` into ``G_c`` (rows ``dE/dw_i``) and writes the per-point gradients.  With ``want_H``, ``H += G_c^T W_c`` on the lower
     tiles (mirrored after the last chunk; ``dE/dK_z = -1/2 L^-T H L^-1``).  With ``want_cross``, the transposed solve turns
-    ``G_c`` into rows ``dE/dk(z, x_i)`` and the rectangular K1-backward adds to ``term_sum``, ``grad_xg`` and ``grad_zg`` (each
-    optional, accumulated).  Returns ``(g_kn [n], g_kd [n] or None, g_ybar [n], H [1, m_pad, m_pad] or None)``.  Device memory:
+    ``G_c`` into rows ``dE/dk(z, x_i)`` and the rectangular K1-backward adds to ``term_sum``, ``grad_xg``, ``grad_zg`` and
+    ``param_sum`` (each optional, accumulated).  Returns ``(g_kn [n], g_kd [n] or None, g_ybar [n], H [1, m_pad, m_pad] or None)``.  Device memory:
     four ``chunk x m_pad`` buffers and three ``m_pad x m_pad`` ones."""
-    _require_cuda(xg, zg, kdiag, kn, ybar, term_sum, grad_xg, grad_zg)
+    _require_cuda(xg, zg, kdiag, kn, ybar, term_sum, grad_xg, grad_zg, param_sum)
     meth = SPARSE_METHOD[method]
     m, m_pad, dt, dev = ch_z.n, ch_z.n_pad, ch_z.dtype, ch_z.device
     n, d = xg.shape[2], xg.shape[3]
@@ -726,7 +727,7 @@ def sparse_elbo_bwd(flat, xg, zg, ch_z, ch_A, s, kdiag, kn, ybar, method, chunk,
         if want_cross:
             ch_z.solve_many_rows_t_(Uc)
             gx = torch.zeros_like(xc) if grad_xg is not None else None
-            kernel_cross_bwd(flat, xc, zg, W=Uc, term_sum=term_sum, grad_xsg=gx, grad_xg=grad_zg)
+            kernel_cross_bwd(flat, xc, zg, W=Uc, term_sum=term_sum, grad_xsg=gx, grad_xg=grad_zg, param_sum=param_sum)
             if gx is not None:
                 grad_xg[:, :, a:b] += gx
     if want_H:

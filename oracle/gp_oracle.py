@@ -42,6 +42,9 @@ __all__ = [
     "logdet",
     "iqf",
     "iqf_diag",
+    "ratio",
+    "entropy",
+    "kl_terms",
     "normal_logpdf",
     "fdd_logpdf",
     "posterior",
@@ -249,7 +252,27 @@ def chol_eps(K, eps=EPSILON):
     (``stheno/random.py:274-276`` via ``B.logdet`` / ``B.iqf_diag``; README.md:820-830)."""
     K = np.asarray(K)
     n = K.shape[-1]
-    return np.linalg.cholesky(K + eps * np.eye(n, dtype=K.dtype))
+    A = K + eps * np.eye(n, dtype=K.dtype)
+    return np.linalg.cholesky(A) if A.ndim != 2 or n <= CHOL_BLOCK else _blocked_cholesky(A)
+
+
+#: Largest order factorised by one ``np.linalg.cholesky`` call.  NumPy 2.3's bundled OpenBLAS (scipy-openblas64 0.3.30)
+#: segfaults in that call at n = 32768 (the C5 joint of ``tests/test_full_size_parity.py``); n = 16384 is fine.
+CHOL_BLOCK = 16384
+
+
+def _blocked_cholesky(A):
+    """Lower Cholesky factor of one SPD matrix ``A`` (overwritten), right-looking over blocks of ``CHOL_BLOCK`` columns:
+    factor the diagonal block, solve the panel below it, subtract its product from the trailing matrix."""
+    n = A.shape[-1]
+    for k in range(0, n, CHOL_BLOCK):
+        e = min(n, k + CHOL_BLOCK)
+        A[k:e, k:e] = np.linalg.cholesky(A[k:e, k:e])
+        A[k:e, e:] = 0.0
+        if e < n:
+            A[e:, k:e] = sla.solve_triangular(A[k:e, k:e], A[e:, k:e].T, lower=True).T  # A21 L11^-T
+            A[e:, e:] -= A[e:, k:e] @ A[e:, k:e].T
+    return A
 
 
 def logdet(K, eps=EPSILON):
@@ -280,6 +303,29 @@ def iqf_diag(K, b, c=None, eps=EPSILON, L=None):
     lb = _tri(L, b)
     lc = lb if c is None else _tri(L, c)
     return np.sum(lb * lc, axis=-2)
+
+
+def ratio(A, Bm, eps=EPSILON):
+    """``B.ratio(A, B)`` = ``tr(B^-1 A)`` = ``tr(L^-1 (L^-1 A)^T)`` with ``L = chol(B + eps I)``
+    (``stheno/model/observations.py:310``, ``stheno/random.py:301``)."""
+    L = chol_eps(Bm, eps)
+    X = _tri(L, np.asarray(A, np.float64))
+    return np.trace(_tri(L, np.swapaxes(X, -1, -2)), axis1=-2, axis2=-1)
+
+
+def entropy(K, eps=EPSILON):
+    """``Normal(K).entropy()`` = ``(logdet K + n (log 2 pi + 1)) / 2`` (``stheno/random.py:282-291``)."""
+    n = np.shape(K)[-1]
+    return (logdet(K, eps) + n * (LOG_2_PI + 1)) / 2
+
+
+def kl_terms(mean_p, K_p, mean_q, K_q, eps_p=EPSILON, eps_q=EPSILON):
+    """The five terms of ``2 KL(p || q)`` (``stheno/random.py:293-309``): ``iqf_diag(K_q, d)``, ``ratio(K_p, K_q)``,
+    ``logdet K_q``, ``-logdet K_p`` and ``-n``, with ``d = mean_q - mean_p`` a column ``[..., n, 1]``."""
+    d = np.asarray(mean_q, np.float64) - np.asarray(mean_p, np.float64)
+    n = np.shape(K_p)[-1]
+    return (iqf_diag(K_q, d, eps=eps_q)[..., 0], ratio(K_p, K_q, eps_q), logdet(K_q, eps_q), -logdet(K_p, eps_p),
+            -float(n))
 
 
 # --------------------------------------------------------------------------------------

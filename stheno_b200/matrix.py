@@ -622,14 +622,28 @@ def cholesky(a):
     return _densify(a).chol()
 
 
+def _raw(route, value, *objs):
+    """``value`` of a raw-pointer route (factorisation, solves, Schur-complement GEMM), which carries no graph or a wrong one:
+    under grad mode, attached to the tensors of ``objs`` that require grad by a node whose backward raises, so that a
+    gradient through it fails instead of coming out silently wrong.  The value itself is unchanged."""
+    from .kernels import _grad_tensors
+
+    ts = _grad_tensors(*objs)
+    if not ts:
+        return value
+    from .autograd import no_gradient
+
+    return no_gradient(route, value, ts)
+
+
 def logdet(a):
     """``B.logdet`` -> ``[...]`` (``stheno/random.py:274``, ``stheno/model/observations.py:334``)."""
     if isinstance(a, Diagonal):
         return torch.log(a.diag).sum(-1)
     if isinstance(a, Woodbury):  # det(D + U U^T) = det(D) det(I + U^T D^-1 U)
-        return torch.log(a.diag_m.diag).sum(-1) + logdet(a.schur())
-    a = _densify(a)
-    return a.chol().logdet.reshape(a.shape[:-2])
+        return _raw("B.logdet", torch.log(a.diag_m.diag).sum(-1) + logdet(a.schur()), a)
+    d = _densify(a)
+    return _raw("B.logdet", d.chol().logdet.reshape(d.shape[:-2]), a)
 
 
 def _rows(t):
@@ -645,12 +659,11 @@ def iqf_diag(a, b, c=None):
         return (b * c / a.diag.unsqueeze(-1)).sum(-2)
     if isinstance(a, Woodbury):
         return torch.diagonal(iqf(a, b, c), dim1=-2, dim2=-1)
-    a = _densify(a)
-    ch = a.chol()
+    ch = _densify(a).chol()
     bt, bs = _rows(b)
     hb = ch.half_solve(bt.contiguous())
     hc = hb if c is None or c is b else ch.half_solve(_rows(c)[0].contiguous())
-    return (hb * hc).sum(-1).reshape(bs + (hb.shape[1],))
+    return _raw("B.iqf_diag", (hb * hc).sum(-1).reshape(bs + (hb.shape[1],)), a, b, c)
 
 
 def iqf(a, b, c=None):
@@ -665,14 +678,13 @@ def iqf(a, b, c=None):
         U = a.lr.left
         ub = U.transpose(-1, -2) @ (b * dinv)  # [..., r, kb]
         uc = ub if c is b else U.transpose(-1, -2) @ (c * dinv)
-        return b.transpose(-1, -2) @ (c * dinv) - iqf(a.schur(), ub, uc)
-    a = _densify(a)
-    ch = a.chol()
+        return _raw("B.iqf", b.transpose(-1, -2) @ (c * dinv) - iqf(a.schur(), ub, uc), a, b, c)
+    ch = _densify(a).chol()
     bt, bs = _rows(b)
     hb = ch.half_solve(bt.contiguous())
     hc = hb if c is None or c is b else ch.half_solve(_rows(c)[0].contiguous())
     out = hb @ hc.transpose(1, 2)
-    return out.reshape(bs + tuple(out.shape[1:]))
+    return _raw("B.iqf", out.reshape(bs + tuple(out.shape[1:])), a, b, c)
 
 
 def ratio(a, b):
@@ -680,12 +692,14 @@ def ratio(a, b):
     if isinstance(a, Diagonal) and isinstance(b, Diagonal):
         return (a.diag / b.diag).sum(-1)
     if isinstance(b, Diagonal):
-        return (diag(a) / b.diag).sum(-1)
-    bm = as_matrix(b)
+        out = (diag(a) / b.diag).sum(-1)
+        # the diagonal of a symbolic kernel matrix comes from the raw-pointer K1 diagonal
+        return _raw("B.ratio", out, a, b) if isinstance(a, KernelDense) and a._mat is None else out
+    bm = _densify(b)
     ch = bm.chol()
     am = dense(a)
     sol = ch.full_solve(_rows(am)[0].contiguous())  # rows: (b^-1 a_col)^T
-    return torch.diagonal(sol, dim1=1, dim2=2).sum(-1).reshape(bm.shape[:-2])
+    return _raw("B.ratio", torch.diagonal(sol, dim1=1, dim2=2).sum(-1).reshape(bm.shape[:-2]), a, b)
 
 
 def block_diag(*ms):

@@ -120,6 +120,44 @@ def test_gemm_nt(ops, dtype, tol):
                 assert blk.abs().max().item() == 0.0
 
 
+@pytest.mark.parametrize("K", [16, 48, 96, 144])
+def test_gemm_nt_f32_ffma(ops, K):
+    """The fp32 FFMA kernel (``gemm_nt_f32_kernel``): the 3xTF32 kernel takes only K >= 128 with K % 32 == 0, so these K
+    (the Schur-complement GEMM of a fp32 Woodbury matrix with n <= 96 has K = round_up(n, 32) < 128) run on FFMA.
+    alpha / beta, beta = 0 over a NaN-filled C, lower mode with a sentinel above the diagonal tiles, batch 2.
+    Bound: 2 K u_32 |alpha| |A| |B|^T plus the rounding of the result and of beta C."""
+    u = 2.0**-24
+    g = torch.Generator(device="cuda").manual_seed(K)
+    A = torch.randn(2, 384, K, device="cuda", generator=g) * torch.exp(torch.randn(2, 384, 1, device="cuda", generator=g))
+    Bm = torch.randn(2, 256, K, device="cuda", generator=g)
+    C0 = torch.randn(2, 384, 256, device="cuda", generator=g)
+    Ad, Bd, Cd = A.double(), Bm.double(), C0.double()
+    absprod = Ad.abs() @ Bd.abs().transpose(1, 2)
+
+    def check(out, alpha, beta, mask=None):
+        ref = alpha * (Ad @ Bd.transpose(1, 2)) + (beta * Cd if beta else 0.0)
+        bound = 2 * K * u * abs(alpha) * absprod + 2 * u * (ref.abs() + abs(beta) * Cd.abs())
+        ok = (out.double() - ref).abs() <= bound
+        assert (ok if mask is None else ok[:, mask]).all()
+
+    launches = ops.launch_count()
+    check(ops.gemm_nt(A, Bm, C0.clone(), alpha=-1.5, beta=0.5), -1.5, 0.5)
+    assert ops.launch_count() == launches + 1  # one kernel, no split or copy
+    nan_c = torch.full_like(C0, float("nan"))
+    out = ops.gemm_nt(A, Bm, nan_c, alpha=-0.75, beta=0.0)
+    assert out.isfinite().all()
+    check(out, -0.75, 0.0)
+    # lower: the tiles on / below the diagonal get beta C + alpha A B^T, the tiles above keep their sentinel bit for bit
+    tr = torch.arange(384, device="cuda")[:, None] // 128
+    tc = torch.arange(256, device="cuda")[None, :] // 128
+    touched = tc <= tr
+    Cs = torch.where(touched, C0, torch.full_like(C0, 31.25))
+    out = ops.gemm_nt(A, Bm, Cs.clone(), alpha=1.0, beta=1.0, lower=True)
+    assert torch.equal(out[:, ~touched], Cs[:, ~touched])
+    Cd = Cs.double()
+    check(out, 1.0, 1.0, touched)
+
+
 def _spd(n, B=1, seed=0, dtype=torch.float64, cond_shift=None):
     g = torch.Generator(device="cuda").manual_seed(seed)
     A = torch.randn(B, n, n, device="cuda", dtype=torch.float64, generator=g)

@@ -146,8 +146,8 @@ int gpk_kernel_cross_bwd_f32(const gpk_kernel_desc* desc_host, const float* xsg,
 /* fp64 emulation on the INT8 tensor cores (wgmma .s32.s8.s8; Ozaki splitting): every row of an operand is scaled by a
  * power of two and split error-free into `slices` signed 7-bit integers; the slice products are EXACT in int32 and are
  * recombined in fp64.  6 slices: 21 int8 GEMMs, product error ~2^-40 |a||b| (zero-mean); 7 slices: 28 GEMMs, ~2^-47.
- * The fp64 entry points gpk_potrf_f64, gpk_trsm_right_f64, gpk_gemm_nt_f64, gpk_posterior_marginals_f64 and
- * gpk_sparse_accumulate_f64 take it as three trailing arguments (slices, ws, ws_bytes): slices = 0 keeps every product on
+ * The fp64 entry points gpk_potrf_f64, gpk_trsm_right_f64, gpk_gemm_nt_f64, gpk_posterior_marginals_f64,
+ * gpk_sparse_posterior_marginals_f64 and gpk_sparse_accumulate_f64 take it as three trailing arguments (slices, ws, ws_bytes): slices = 0 keeps every product on
  * the fp64 tensor cores (ws may be NULL); slices = 5..8 with a caller-owned, 1024-byte aligned scratch `ws` runs the LARGE
  * GEMM-shaped updates of that call on the int8 tensor cores -- the trailing updates of a factorisation (batch 1,
  * n_pad >= 2048), and products of batch 1 with M, N, K >= 256 and M N K >= 1.5e9 (reductions longer than 65536 in several
@@ -155,7 +155,8 @@ int gpk_kernel_cross_bwd_f32(const gpk_kernel_desc* desc_host, const float* xsg,
  * the fp64 tensor cores.  The size queries give the scratch that makes every update of a call eligible, 0 when none is:
  *   gpk_gemm_nt_oz_ws_bytes     one product M x N x K
  *   gpk_trsm_right_oz_ws_bytes  the largest product of the recursive solve of `rows` right-hand sides (also the solve inside
- *                               gpk_posterior_marginals_f64 (rows = chunk) and gpk_sparse_accumulate_f64 (rows = c_pad))
+ *                               gpk_posterior_marginals_f64 and gpk_sparse_posterior_marginals_f64 (rows = chunk) and
+ *                               gpk_sparse_accumulate_f64 (rows = c_pad))
  *   gpk_potrf_oz_ws_bytes       a factorisation (the panel slices; from n_pad >= 4096 those of a pair of panels)
  * Calls that share a scratch buffer must be stream-ordered with respect to each other. */
 int64_t gpk_gemm_nt_oz_ws_bytes(int64_t M, int64_t N, int64_t K, int32_t slices);
@@ -267,6 +268,26 @@ int gpk_posterior_marginals_f32(const gpk_kernel_desc* desc_host, const float* x
                                 const float* xg, int64_t xg_gstride, int64_t n, int32_t d, const float* L, int64_t ldl,
                                 int64_t n_pad, const float* half_y, float* dot, float* sq, int64_t chunk, float* ws,
                                 int64_t ws_elems, void* stream);
+
+/* The same for a sparse (inducing-point) posterior, PosteriorKernel(z, K_z) + SubspaceKernel(z, A) with PosteriorMean(z, K_z, mu)
+ * (stheno/model/observations.py:255-277), batch 1, at ns test points:
+ *   V^T = k(x*, z) L_z^-T,  U^T = k(x*, z) L_S^-T   (K1 rows once, copied on the device, two right TRSMs)
+ *   dot[i] = <v_i, half_y>;  sq_z[i] = |v_i|^2;  sq_s[i] = |u_i|^2   (fp64 sums in both precisions)
+ * Lz: padded lower factor of K_z + eps I; LS: that of the stored A (= L_z A L_z^T) + eps I; half_y = (L_z^-1 (mu - m_z(z)))^T
+ * zero-padded to m_pad (dot may be NULL: variances only; sq_z and sq_s are always written).  The caller forms
+ * mean = m(x*) + dot and variance = (k(x*, x*) - sq_z) + sq_s.  Test points are walked in chunks of `chunk` rows (multiple of
+ * 128) through `ws` (>= gpk_sparse_posterior_ws_elems(chunk, m_pad) elements, 16-byte aligned): device memory
+ * O(chunk m_pad) whatever ns is.  The emulation scratch of the fp64 entry point: gpk_trsm_right_oz_ws_bytes(m_pad, chunk). */
+int64_t gpk_sparse_posterior_ws_elems(int64_t chunk, int64_t m_pad);
+int gpk_sparse_posterior_marginals_f64(const gpk_kernel_desc* desc_host, const double* xsg, int64_t xsg_gstride, int64_t ns,
+                                       const double* zg, int64_t zg_gstride, int64_t m, int32_t d, const double* Lz,
+                                       int64_t ldlz, const double* LS, int64_t ldls, int64_t m_pad, const double* half_y,
+                                       double* dot, double* sq_z, double* sq_s, int64_t chunk, double* ws, int64_t ws_elems,
+                                       int32_t slices, void* oz_ws, int64_t oz_ws_bytes, void* stream);
+int gpk_sparse_posterior_marginals_f32(const gpk_kernel_desc* desc_host, const float* xsg, int64_t xsg_gstride, int64_t ns,
+                                       const float* zg, int64_t zg_gstride, int64_t m, int32_t d, const float* Lz, int64_t ldlz,
+                                       const float* LS, int64_t ldls, int64_t m_pad, const float* half_y, float* dot,
+                                       float* sq_z, float* sq_s, int64_t chunk, float* ws, int64_t ws_elems, void* stream);
 
 /* Streamed sparse (inducing-point) accumulation -- AbstractPseudoObservations._compute, stheno/model/observations.py:279-336,
  * one chunk of `c` data points per call; K_zx (8.6 GB at n = 262144, m = 4096) is never held.  Per chunk, stream-ordered:

@@ -55,6 +55,8 @@ _SIGNATURES = {
     "gpk_transpose": [_ptr, _i64, _i64, _i64, _i64, _ptr, _i64, _i64, _i32, _ptr],
     "gpk_posterior_marginals": [POINTER(KernelDesc), _ptr, _i64, _i64, _ptr, _i64, _i64, _i32, _ptr, _i64, _i64, _ptr, _ptr, _ptr,
                                 _i64, _ptr, _i64, "OZ", _ptr],
+    "gpk_sparse_posterior_marginals": [POINTER(KernelDesc), _ptr, _i64, _i64, _ptr, _i64, _i64, _i32, _ptr, _i64, _ptr, _i64,
+                                       _i64, _ptr, _ptr, _ptr, _ptr, _i64, _ptr, _i64, "OZ", _ptr],
     "gpk_sparse_accumulate": [POINTER(KernelDesc), _ptr, _i64, _i64, _ptr, _i64, _i64, _i32, _ptr, _i64, _i64, _ptr, _ptr, _ptr,
                               _i32, _ptr, _i64, _ptr, _ptr, _ptr, _i64, "OZ", _ptr],
     "gpk_sparse_rows_bwd": [_i64, _i64, _ptr, _i64, _ptr, _i64, _ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _ptr],
@@ -63,6 +65,7 @@ _PLAIN = {
     "gpk_version": ([], c_int32),
     "gpk_round_up": ([_i64], _i64),
     "gpk_sparse_ws_elems": ([_i64, _i64], _i64),
+    "gpk_sparse_posterior_ws_elems": ([_i64, _i64], _i64),
     "gpk_probe_dmma_tflops": ([], c_double),
     "gpk_debug_leaf_phase_clock": ([_ptr], c_int32),
     "gpk_debug_oz_tile": ([_i32, _i32, _i32, _i32, _i32, POINTER(c_int32), POINTER(c_int32)], c_int32),

@@ -1487,6 +1487,50 @@ def _shared_posterior(mean, kernel):
     )
 
 
+def _sparse_posterior(mean, kernel, x):
+    """The sparse counterpart of :func:`_shared_posterior`: the ``PosteriorMean`` and ``PosteriorKernel + SubspaceKernel`` of
+    one ``PseudoObs*`` problem (``AbstractPseudoObservations``) at numeric, single-output, unbatched ``x``, with one cross
+    kernel that flattens to one descriptor and nothing that requires grad -- the marginals :func:`_sparse_marginals` streams."""
+    if not (isinstance(mean, PosteriorMean) and isinstance(kernel, SumKernel)):
+        return False
+    pk, sk, k = kernel.a, kernel.b, mean.k_zi
+    if not (isinstance(pk, PosteriorKernel) and isinstance(sk, SubspaceKernel)):
+        return False
+    if not (pk.K_z is mean.K_z and pk.z is mean.z and sk.z is mean.z):
+        return False
+    if not (pk.k_zi is k and pk.k_zj is k and sk.k_zi is k and sk.k_zj is k and k.symmetric):
+        return False
+    if _is_multi(x) or _is_multi(mean.z) or as_input(x).batch_shape or as_input(mean.z).batch_shape:
+        return False
+    flat, _ = k._flat()
+    if flat is None or not flat.terms:
+        return False
+    if _grad_tensors(mean, kernel, x):
+        return False
+    return mean.K_z.chol().batch == 1 and sk.A.chol().batch == 1
+
+
+def _sparse_marginals(mean, kernel, x, want_dot):
+    """``(dot, sq_z, sq_s)`` of a posterior :func:`_sparse_posterior` accepts, each ``[..., n, 1]``: the K1 rows at ``x``
+    are formed once per chunk of test points and solved against ``L_z`` and against the factor of ``A`` (``dot`` None unless
+    ``want_dot``)."""
+    xi, zi = as_input(x), as_input(mean.z)
+    flat, scales = mean.k_zi._flat()
+    half_y = mean._half_y()[0] if want_dot else None
+    out = ops.sparse_posterior_marginals(flat, xi.scaled(scales), zi.scaled(scales), mean.K_z.chol(), kernel.b.A.chol(),
+                                         half_y, want_dot=want_dot)
+    return tuple(None if t is None else t.reshape(xi.n, 1) for t in out)
+
+
+def marginal_var(mean, kernel, x):
+    """``k.elwise(x)`` of a posterior process with mean ``mean``, ``[..., n, 1]``: the streamed sparse marginals where
+    :func:`_sparse_posterior` holds, else the kernel's own element-wise evaluation."""
+    if _sparse_posterior(mean, kernel, x):
+        _, sq_z, sq_s = _sparse_marginals(mean, kernel, x, want_dot=False)
+        return (_elwise_any(kernel.a.k_ij, x, None, True) - sq_z) + sq_s
+    return _elwise_any(kernel, x, None, True)
+
+
 def mean_var(mean, kernel, x):
     """``mlkernels.mean_var``: mean ``[..., n, 1]`` (device) and variance (matrix), sharing ``L^-1 k(z, x)`` between
     the two for an exact posterior (``stheno/model/fdd.py:68-70``)."""
@@ -1540,4 +1584,7 @@ def mean_var_diag(mean, kernel, x):
         else:
             dot, sq, _ = _exact_posterior(mean.K_z, route[0], mean._ybar(), fwd, half_y=mean._half_y())
         return prior_m + dot.reshape(shp).unsqueeze(-1), prior_v - sq.reshape(shp).unsqueeze(-1)
+    if _sparse_posterior(mean, kernel, x):
+        dot, sq_z, sq_s = _sparse_marginals(mean, kernel, x, want_dot=True)
+        return mean.m_i.dev(x) + dot, (_elwise_any(kernel.a.k_ij, x, None, True) - sq_z) + sq_s
     return mean.dev(x), _elwise_any(kernel, x, None, True)

@@ -3,7 +3,7 @@ import numpy as np
 import torch
 
 from .. import matrix as M
-from ..kernels import Input, Kernel, _elwise_any, as_input, mean_var, mean_var_diag, num_elements, pairwise
+from ..kernels import Input, Kernel, as_input, marginal_var, mean_var, mean_var_diag, num_elements, pairwise
 from ..random import Normal, RandomProcess
 from .._util import origin_of, to_dev
 
@@ -68,7 +68,7 @@ class FDD(Normal):
             return p.mean.dev(x)
 
         def var_diag():
-            return _elwise_any(p.kernel, x, None, True).squeeze(-1) + M.diag(noise_m)
+            return marginal_var(p.mean, p.kernel, x).squeeze(-1) + M.diag(noise_m)
 
         def mv():
             m, v = mean_var(p.mean, p.kernel, x)

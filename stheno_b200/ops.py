@@ -614,6 +614,40 @@ def posterior_marginals(flat, xsg, xg, chol, half_y=None, want_sq=True, chunk=40
     return dot, sq
 
 
+def sparse_posterior_marginals(flat, xsg, zg, ch_z, ch_s, half_y, want_dot=True, chunk=4096):
+    """The marginals of a sparse posterior in one call (``gpk_sparse_posterior_marginals``): ``(dot [n*] or None, sq_z [n*],
+    sq_s [n*])`` with ``V^T = k(x*, z) L_z^-T``, ``U^T = k(x*, z) L_S^-T``, ``dot = V^T half_y``, ``sq_z = |v_i|^2``,
+    ``sq_s = |u_i|^2``.  ``ch_z``: factor of ``K_z``; ``ch_s``: factor of the stored ``A`` (``L_z A L_z^T``) + eps I.  One
+    problem (no batch); test points streamed in chunks of ``chunk`` rows through two ``chunk x m_pad`` buffers."""
+    _check_groups(zg, flat)
+    _require_cuda(xsg, zg, half_y)
+    if ch_z.batch != 1 or ch_s.batch != 1 or xsg.shape[1] != 1 or zg.shape[1] != 1:
+        raise ValueError("sparse_posterior_marginals handles a single problem")
+    if ch_s.n_pad != ch_z.n_pad or zg.shape[2] != ch_z.n:
+        raise ValueError("sparse_posterior_marginals: the factors and the inducing points do not match")
+    xsg, zg = xsg.contiguous(), zg.contiguous()
+    ns, d = xsg.shape[2], xsg.shape[3]
+    dt, dev, m_pad = ch_z.dtype, ch_z.device, ch_z.n_pad
+    dot = torch.empty(ns, dtype=dt, device=dev) if want_dot else None
+    sq_z = torch.empty(ns, dtype=dt, device=dev)
+    sq_s = torch.empty(ns, dtype=dt, device=dev)
+    if ns == 0:
+        return dot, sq_z, sq_s
+    chunk = min(round_up(chunk), round_up(ns))
+    lib = _lib.load()
+    ws = torch.empty(int(lib.gpk_sparse_posterior_ws_elems(chunk, m_pad)), dtype=dt, device=dev)
+    em = _emulation(dt, dev, lambda lib, s: lib.gpk_trsm_right_oz_ws_bytes(m_pad, chunk, s))
+    Lz, Ls = ch_z.L_padded(), ch_s.L_padded()
+    hy = half_y.contiguous() if want_dot else None
+    desc = flat.desc()
+    rc = _fn("gpk_sparse_posterior_marginals", dt)(
+        ctypes.byref(desc), _ptr(xsg), xsg.stride(0), ns, _ptr(zg), zg.stride(0), ch_z.n, d, _ptr(Lz), Lz.stride(1), _ptr(Ls),
+        Ls.stride(1), m_pad, _ptr(hy), _ptr(dot), _ptr(sq_z), _ptr(sq_s), chunk, _ptr(ws), ws.numel(), *em, _stream(),
+    )
+    check(rc, "gpk_sparse_posterior_marginals")
+    return dot, sq_z, sq_s
+
+
 SPARSE_METHOD = {"vfe": 0, "fitc": 1, "dtc": 2}
 
 

@@ -267,10 +267,32 @@ def test_transpose_and_symmetrize(ops):
     assert torch.equal(ops.symmetrize_(S.clone(), 100), ref)
 
 
+def tc32_probe(ops, M, N, K, batch=1, lower=False, gemm=None):
+    """Which kernel an fp32 ``gemm_nt`` of this shape runs on: "tc32" (3xTF32 wgmma) or "ffma".
+
+    The probe puts a single ``a = 1 + 2^-11`` at the same k in the last row of A and the first row of B (a tile on or below
+    the diagonal).  The 3xTF32 split drops the ``a_lo b_lo`` term and gives exactly ``a^2 - 2^-22 = 1 + 2^-10``; FFMA gives
+    ``a^2 = 1 + 2^-10 + 2^-22`` exactly.  A kernel that silently falls back to FFMA therefore shows here."""
+    gemm = ops.gemm_nt if gemm is None else gemm
+    A = torch.zeros(batch, M, K, device="cuda", dtype=torch.float32)
+    Bm = torch.zeros(batch, N, K, device="cuda", dtype=torch.float32)
+    a = 1.0 + 2.0**-11
+    A[:, M - 1, K - 1] = a
+    Bm[:, 0, K - 1] = a
+    C = gemm(A, Bm, torch.zeros(batch, M, N, device="cuda", dtype=torch.float32), alpha=-1.0, beta=1.0, lower=lower)
+    got = {float(v) for v in C[:, M - 1, 0].cpu()}
+    if got == {-(1.0 + 2.0**-10)}:
+        return "tc32"
+    assert got == {-(1.0 + 2.0**-10 + 2.0**-22)}, got
+    return "ffma"
+
+
 @pytest.mark.parametrize("M,N,K,batch,lower", [(128, 128, 128, 1, False), (256, 384, 512, 2, False), (384, 384, 256, 3, True),
                                                  (1024, 512, 1024, 1, False)])
 def test_gemm_f32_tensor_core_3xtf32(ops, M, N, K, batch, lower):
-    """fp32 GEMM on wgmma (3xTF32 split): fp32-level accuracy against an fp64 reference, incl. strided views."""
+    """fp32 GEMM on wgmma (3xTF32 split): fp32-level accuracy against an fp64 reference, incl. strided views; the probe proves
+    the shape runs on the 3xTF32 kernel (FFMA would pass the accuracy bar too)."""
+    assert tc32_probe(ops, M, N, K, batch, lower) == "tc32"
     g = torch.Generator(device="cuda").manual_seed(M + N + K)
     big = torch.randn(batch, M + 128, K + 64, device="cuda", generator=g)
     A = big[:, 64:64 + M, 32:32 + K]  # a strided view: ld = K + 64, non-zero offset

@@ -14,6 +14,9 @@ NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
+    # a non-static function needs an earlier declaration (common.cuh, gpk.h): one whose definition drifts from it fails
+    # to compile instead of leaving an undefined symbol that only loading the library reports
+    "-Xcompiler", "-Werror=missing-declarations",
     "--expt-relaxed-constexpr",
 ]
 

@@ -1,4 +1,4 @@
-// Shared device helpers for libgpk (sm_90a only).
+// Shared helpers for libgpk (sm_90a only), and the host functions one translation unit calls in another.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -12,10 +12,12 @@ namespace gpk {
 
 extern long long g_launch_count;  // defined in util.cu
 
-#define GPK_CHECK_LAUNCH()                                   \
-  do {                                                       \
-    cudaError_t e__ = cudaGetLastError();                    \
-    if (e__ != cudaSuccess) return -1000 - (int)e__;         \
+// a CUDA runtime result as a libgpk return code: 0, or -1000 - the cudaError_t (gpk.h)
+inline int cuda_rc(cudaError_t e) { return e == cudaSuccess ? 0 : -1000 - (int)e; }
+
+#define GPK_CHECK_LAUNCH()                                                  \
+  do {                                                                      \
+    if (const int rc__ = ::gpk::cuda_rc(cudaGetLastError())) return rc__; \
   } while (0)
 
 #define GPK_COUNT_LAUNCH() (++::gpk::g_launch_count)
@@ -28,16 +30,32 @@ int opt_in_smem(int bytes) {
   static std::atomic<int> set[64];  // by device ordinal
   static std::mutex mu;             // never lowers a size another host thread has just set
   int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return -1000 - (int)e;
+  if (const int rc = cuda_rc(cudaGetDevice(&dev))) return rc;
   if (dev >= 64) return GPK_ERR_UNSUPPORTED;
   if (bytes <= set[dev].load(std::memory_order_acquire)) return 0;
   std::lock_guard<std::mutex> lock(mu);
   if (bytes <= set[dev].load(std::memory_order_relaxed)) return 0;
-  e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) return -1000 - (int)e;
+  if (const int rc = cuda_rc(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes))) return rc;
   set[dev].store(bytes, std::memory_order_release);
   return 0;
+}
+
+// exp, sqrt, rsqrt and log of a T: the fp64 or the fp32 library function
+template <typename T>
+__device__ __forceinline__ T t_exp(T v) {
+  return sizeof(T) == 8 ? (T)exp((double)v) : (T)expf((float)v);
+}
+template <typename T>
+__device__ __forceinline__ T t_sqrt(T v) {
+  return sizeof(T) == 8 ? (T)sqrt((double)v) : (T)sqrtf((float)v);
+}
+template <typename T>
+__device__ __forceinline__ T t_rsqrt(T v) {
+  return sizeof(T) == 8 ? (T)rsqrt((double)v) : (T)rsqrtf((float)v);
+}
+template <typename T>
+__device__ __forceinline__ T t_log(T v) {
+  return sizeof(T) == 8 ? (T)log((double)v) : (T)logf((float)v);
 }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -125,15 +143,73 @@ __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double
                : "d"(a), "d"(b));
 }
 
-// The int8-slice emulation arguments (slices, ws, ws_bytes) of the fp64 entry points: slices 0 (fp64 tensor cores) or 5..8
-// with a 1024-byte aligned scratch.  0 or GPK_ERR_ARG (gemm_oz.cu).
-int oz_check_emulation(int32_t slices, const void* ws);
-
 template <typename T>
 __device__ __forceinline__ T warp_sum(T v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+
+// ---- host functions that one translation unit calls in another ----------------------------------------------------------
+// Each is defined in the file named above it, on the caller's stream, and returns 0 or a negative gpk.h error code unless
+// its comment says otherwise.  (S, ws, ws_bytes) are the int8-slice emulation arguments of gpk.h's fp64 entry points; the
+// fp32 overloads ignore them.
+
+// kernel_matrix.cu: out[i][j] = k(x_i, y_j) for one problem, no noise or jitter, zero padded to multiples of 128
+int kernel_rows(const gpk_kernel_desc* desc, const double* xg, int64_t xg_gstride, int64_t n, const double* yg,
+                int64_t yg_gstride, int64_t n2, int32_t d, double* out, int64_t ldo, cudaStream_t stream);
+int kernel_rows(const gpk_kernel_desc* desc, const float* xg, int64_t xg_gstride, int64_t n, const float* yg,
+                int64_t yg_gstride, int64_t n2, int32_t d, float* out, int64_t ldo, cudaStream_t stream);
+
+// util.cu: dot[r] = <V[r, :n_cols], b> and sq[r] = |V[r, :n_cols]|^2 for r < rows, one matrix; dot or sq may be null
+int row_dot_sq(const double* V, int64_t ldv, int64_t rows, int64_t n_cols, const double* b, double* dot, double* sq,
+               cudaStream_t stream);
+int row_dot_sq(const float* V, int64_t ldv, int64_t rows, int64_t n_cols, const float* b, float* dot, float* sq,
+               cudaStream_t stream);
+
+// gemm.cu: C = beta C + alpha A B^T (gpk_gemm_nt_f64 / _f32)
+int gemm_nt(int64_t M, int64_t N, int64_t K, double alpha, const double* A, int64_t lda, int64_t a_bs, const double* B,
+            int64_t ldb, int64_t b_bs, double beta, double* C, int64_t ldc, int64_t c_bs, int32_t lower, int32_t batch,
+            int32_t S, void* ws, int64_t ws_bytes, cudaStream_t stream);
+int gemm_nt(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t lda, int64_t a_bs, const float* B,
+            int64_t ldb, int64_t b_bs, float beta, float* C, int64_t ldc, int64_t c_bs, int32_t lower, int32_t batch,
+            int32_t S, void* ws, int64_t ws_bytes, cudaStream_t stream);
+// gemm.cu: the in-situ event profile of the fp64 GEMMs (gpk_gemm_profile_*); kind 0 = DMMA, 1 = int8-slice emulation
+bool prof_enabled();
+void prof_begin(cudaStream_t stream, double flops, int kind);
+void prof_end(cudaStream_t stream);
+
+// potrf.cu: X L^T = B in place for one matrix (gpk_trsm_right_f64 / _f32)
+int trsm_right(const double* L, int64_t ldl, int64_t n_pad, double* B, int64_t ldb, int64_t rows, int32_t S, void* ws,
+               int64_t ws_bytes, cudaStream_t stream);
+int trsm_right(const float* L, int64_t ldl, int64_t n_pad, float* B, int64_t ldb, int64_t rows, int32_t S, void* ws,
+               int64_t ws_bytes, cudaStream_t stream);
+
+// gemm_oz.cu: the emulation arguments of an fp64 entry point are valid: S = 0 (fp64 tensor cores), or 5..8 with a
+// 1024-byte aligned scratch.  0 or GPK_ERR_ARG
+int oz_check_emulation(int32_t S, const void* ws);
+// gemm_oz.cu: scratch bytes of the S int8 slices of `rows` rows of K columns, with their row exponents
+int64_t oz_ws_bytes(int64_t rows, int64_t K, int32_t S);
+// gemm_oz.cu: slices of the rows x K panel P into ws, laid out for cap_rows rows
+int oz_slice_panel(const double* P, int64_t ldp, int64_t rows, int64_t K, void* ws, int64_t cap_rows, int32_t S,
+                   cudaStream_t stream);
+// gemm_oz.cu: C[M x N] = beta C + alpha A B^T, A = sliced rows [rowA, rowA + M) of wsA, B = sliced rows [rowB, rowB + N) of wsB
+int oz_gemm_sliced(int64_t M, int64_t N, int64_t K, double alpha, const void* wsA, int64_t capA, int64_t rowA,
+                   const void* wsB, int64_t capB, int64_t rowB, double beta, double* C, int64_t ldc, int32_t lower,
+                   int32_t S, cudaStream_t stream);
+// gemm_oz.cu: gemm_nt on the int8 tensor cores.  1 = done, 0 = not applicable (the caller uses DMMA), < 0 = error
+int gemm_nt_f64_emulated(int64_t M, int64_t N, int64_t K, double alpha, const double* A, int64_t lda, const double* B,
+                         int64_t ldb, double beta, double* C, int64_t ldc, int32_t lower, int32_t S, void* ws,
+                         int64_t ws_bytes, cudaStream_t stream);
+
+// gemm_tc32.cu: fp32 gemm_nt on the tensor cores (wgmma, 3xTF32).  1 = launched, 0 = shape not supported (the caller uses
+// the FFMA kernel), < 0 = error
+int gemm_nt_f32_tc(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t lda, int64_t a_bs, const float* B,
+                   int64_t ldb, int64_t b_bs, float beta, float* C, int64_t ldc, int64_t c_bs, int32_t lower,
+                   int32_t batch, cudaStream_t stream);
+// gemm_tc32.cu: C[M x N] (fp64, lower tiles) -= P[0:M] P[0:N]^T, P = the M x K fp32 panel ws_rows (convert_panel_f32)
+int syrk_f64_tf32x3(int64_t M, int64_t N, int64_t K, const float* ws_rows, double* C, int64_t ldc, cudaStream_t stream);
+// gemm_tc32.cu: ws (rows x K, dense) = the fp64 panel P rounded to fp32
+int convert_panel_f32(const double* P, int64_t ldp, int64_t rows, int64_t K, float* ws, cudaStream_t stream);
 
 }  // namespace gpk

@@ -468,7 +468,7 @@ struct GemmProfile {
 static GemmProfile g_prof;
 
 bool prof_enabled() { return g_prof.enabled; }
-void prof_begin(cudaStream_t s, double flops, int kind = 0) {
+void prof_begin(cudaStream_t s, double flops, int kind) {
   cudaEvent_t a, b;
   if (cudaEventCreate(&a) != cudaSuccess || cudaEventCreate(&b) != cudaSuccess) return;
   g_prof.ev.push_back(a);
@@ -479,12 +479,9 @@ void prof_begin(cudaStream_t s, double flops, int kind = 0) {
 }
 void prof_end(cudaStream_t s) { cudaEventRecord(g_prof.ev.back(), s); }
 
-int gemm_nt_f64_emulated(int64_t, int64_t, int64_t, double, const double*, int64_t, const double*, int64_t, double, double*,
-                         int64_t, int32_t, int32_t, void*, int64_t, cudaStream_t);  // gemm_oz.cu: 1 = done, 0 = not applicable, < 0 error
-
-int gemm_nt_f64(int64_t M, int64_t N, int64_t K, double alpha, const double* A, int64_t lda, int64_t a_bs,
-                const double* B, int64_t ldb, int64_t b_bs, double beta, double* C, int64_t ldc, int64_t c_bs,
-                int32_t lower, int32_t batch, int32_t slices, void* ws, int64_t ws_bytes, cudaStream_t stream) {
+int gemm_nt(int64_t M, int64_t N, int64_t K, double alpha, const double* A, int64_t lda, int64_t a_bs, const double* B,
+            int64_t ldb, int64_t b_bs, double beta, double* C, int64_t ldc, int64_t c_bs, int32_t lower, int32_t batch,
+            int32_t slices, void* ws, int64_t ws_bytes, cudaStream_t stream) {
   int rc = check_gemm_args<double>(M, N, K, A, lda, B, ldb, C, ldc, batch);
   if (!rc) rc = oz_check_emulation(slices, ws);
   if (rc) return rc;
@@ -504,7 +501,7 @@ int gemm_nt_f64(int64_t M, int64_t N, int64_t K, double alpha, const double* A, 
     if (g_prof.enabled) {
       const double tn = (double)tiles_n, tmm = (double)tiles_m;
       const double tiles = lower ? (tn * (tn + 1) / 2 + (tmm - tn) * tn) : tmm * tn;  // in 128 x 128 units
-      prof_begin(stream, tiles * 2.0 * GM_BM * GM_BN * (double)K * batch);
+      prof_begin(stream, tiles * 2.0 * GM_BM * GM_BN * (double)K * batch, 0);
     }
     gemm_nt_f64_v3_kernel<32, 2><<<grid3, G3_THREADS, smem, stream>>>(p3);
     if (g_prof.enabled) prof_end(stream);
@@ -541,12 +538,9 @@ int gemm_nt_f64(int64_t M, int64_t N, int64_t K, double alpha, const double* A, 
   return 0;
 }
 
-int gemm_nt_f32_tc(int64_t, int64_t, int64_t, float, const float*, int64_t, int64_t, const float*, int64_t, int64_t, float,
-                   float*, int64_t, int64_t, int32_t, int32_t, cudaStream_t);  // gemm_tc32.cu (wgmma 3xTF32)
-
-int gemm_nt_f32(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t lda, int64_t a_bs,
-                const float* B, int64_t ldb, int64_t b_bs, float beta, float* C, int64_t ldc, int64_t c_bs,
-                int32_t lower, int32_t batch, cudaStream_t stream) {
+int gemm_nt(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t lda, int64_t a_bs, const float* B,
+            int64_t ldb, int64_t b_bs, float beta, float* C, int64_t ldc, int64_t c_bs, int32_t lower, int32_t batch, int32_t,
+            void*, int64_t, cudaStream_t stream) {
   int rc = check_gemm_args<float>(M, N, K, A, lda, B, ldb, C, ldc, batch);
   if (rc) return rc;
   if (M == 0 || N == 0) return 0;
@@ -580,8 +574,7 @@ static int profile_read_kind(int kind, double* total_ms, double* total_flops, in
   for (size_t i = 0; i < n; ++i) {
     if (kind >= 0 && gpk::g_prof.kind[i] != kind) continue;
     float t = 0.f;
-    cudaError_t e = cudaEventElapsedTime(&t, gpk::g_prof.ev[2 * i], gpk::g_prof.ev[2 * i + 1]);
-    if (e != cudaSuccess) return -1000 - (int)e;
+    if (const int rc = gpk::cuda_rc(cudaEventElapsedTime(&t, gpk::g_prof.ev[2 * i], gpk::g_prof.ev[2 * i + 1]))) return rc;
     ms += t;
     fl += gpk::g_prof.flops[i];
     ++cnt;
@@ -601,13 +594,13 @@ int gpk_gemm_nt_f64(int64_t M, int64_t N, int64_t K, double alpha, const double*
                     const double* B, int64_t ldb, int64_t b_bstride, double beta, double* C, int64_t ldc,
                     int64_t c_bstride, int32_t lower, int32_t batch, int32_t slices, void* ws, int64_t ws_bytes,
                     void* stream) {
-  return gpk::gemm_nt_f64(M, N, K, alpha, A, lda, a_bstride, B, ldb, b_bstride, beta, C, ldc, c_bstride, lower, batch,
-                          slices, ws, ws_bytes, (cudaStream_t)stream);
+  return gpk::gemm_nt(M, N, K, alpha, A, lda, a_bstride, B, ldb, b_bstride, beta, C, ldc, c_bstride, lower, batch, slices,
+                      ws, ws_bytes, (cudaStream_t)stream);
 }
 int gpk_gemm_nt_f32(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t lda, int64_t a_bstride,
                     const float* B, int64_t ldb, int64_t b_bstride, float beta, float* C, int64_t ldc,
                     int64_t c_bstride, int32_t lower, int32_t batch, void* stream) {
-  return gpk::gemm_nt_f32(M, N, K, alpha, A, lda, a_bstride, B, ldb, b_bstride, beta, C, ldc, c_bstride, lower, batch,
-                          (cudaStream_t)stream);
+  return gpk::gemm_nt(M, N, K, alpha, A, lda, a_bstride, B, ldb, b_bstride, beta, C, ldc, c_bstride, lower, batch, 0,
+                      nullptr, 0, (cudaStream_t)stream);
 }
 }

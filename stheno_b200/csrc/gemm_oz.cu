@@ -42,10 +42,6 @@
 #include "wgmma.cuh"
 
 namespace gpk {
-bool prof_enabled();  // gemm.cu: in-situ event profile (bench.py's roofline)
-void prof_begin(cudaStream_t, double flops, int kind);
-void prof_end(cudaStream_t);
-
 namespace {
 
 constexpr int OZ_BM = 128, OZ_BN = 64, OZ_BK = 64;  // BK in bytes = int8 elements
@@ -432,23 +428,9 @@ oz_slice_kernel(const double* __restrict__ P, int64_t ldp, int64_t rows, int32_t
   }
 }
 
-typedef CUresult (*OzEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-OzEncodeTiledFn oz_encode_fn() {
-  static OzEncodeTiledFn fn = [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess)
-      return (OzEncodeTiledFn) nullptr;
-    return (OzEncodeTiledFn)p;
-  }();
-  return fn;
-}
-
-bool oz_make_map(CUtensorMap* m, const int8_t* planes, int64_t K, int64_t rows_cap, int64_t plane_stride, int S,
-                 int box_rows) {
-  OzEncodeTiledFn enc = oz_encode_fn();
+static bool oz_make_map(CUtensorMap* m, const int8_t* planes, int64_t K, int64_t rows_cap, int64_t plane_stride, int S,
+                        int box_rows) {
+  const EncodeTiledFn enc = encode_tiled_fn();
   if (!enc) return false;
   cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)rows_cap, (cuuint64_t)S};
   cuuint64_t strides[2] = {(cuuint64_t)K, (cuuint64_t)plane_stride};
@@ -465,8 +447,7 @@ int oz_launch_slice(const double* P, int64_t ldp, int64_t rows, int64_t K, int8_
   if (rows == 0) return 0;
   oz_slice_kernel<S><<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(P, ldp, rows, (int32_t)K, planes, plane_stride, ex);
   GPK_COUNT_LAUNCH();
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : -1000 - (int)e;
+  return cuda_rc(cudaGetLastError());
 }
 
 // C *= beta on the elements the GEMM kernel writes: all of C, or in lower mode the tiles that touch the lower triangle
@@ -521,10 +502,9 @@ int oz_launch_gemm(int64_t M, int64_t N, int64_t K, double alpha, const int8_t* 
   cfg.numAttrs = 1;
   const cudaError_t le = cudaLaunchKernelEx(&cfg, oz_gemm_kernel<S>, mA, mB, p);
   if (prof_enabled()) prof_end(stream);
-  if (le != cudaSuccess) return -1000 - (int)le;
+  if (const int rc = cuda_rc(le)) return rc;
   GPK_COUNT_LAUNCH();
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : -1000 - (int)e;
+  return cuda_rc(cudaGetLastError());
 }
 
 }  // namespace
@@ -613,7 +593,6 @@ static int oz_gemm(int64_t M, int64_t N, int64_t K, double alpha, const double* 
   return 0;
 }
 
-// 1 = done on the emulated path, 0 = not applicable (caller uses DMMA), < 0 = error
 int gemm_nt_f64_emulated(int64_t M, int64_t N, int64_t K, double alpha, const double* A, int64_t lda, const double* B,
                          int64_t ldb, double beta, double* C, int64_t ldc, int32_t lower, int32_t S, void* ws, int64_t ws_bytes,
                          cudaStream_t stream) {

@@ -179,23 +179,9 @@ gemm_nt_f32_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_con
 }
 
 // ---- host ------------------------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess) return (EncodeTiledFn) nullptr;
-    return (EncodeTiledFn)p;
-  }();
-  return fn;
-}
-
 static bool make_map(CUtensorMap* m, const float* base, int64_t K, int64_t rows, int64_t ld, int64_t bs, int32_t batch,
                      int box_rows) {
-  EncodeTiledFn enc = encode_fn();
+  const EncodeTiledFn enc = encode_tiled_fn();
   if (!enc) return false;
   cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)rows, (cuuint64_t)batch};
   cuuint64_t strides[2] = {(cuuint64_t)ld * 4, (cuuint64_t)((batch > 1) ? bs : rows * ld) * 4};
@@ -217,12 +203,10 @@ static int launch_tc(int64_t M, int64_t N, int64_t K, float alpha, const float* 
   dim3 grid((unsigned)(p.tiles_m * p.tiles_n), (unsigned)batch);
   gemm_nt_f32_tc_kernel<CT><<<grid, TC_GEMM_THREADS, TC_SMEM_BYTES, stream>>>(mA, mB, p);
   GPK_COUNT_LAUNCH();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return -1000 - (int)e;
+  if (const int rc = cuda_rc(cudaGetLastError())) return rc;
   return 1;
 }
 
-// returns 1 if the problem was launched on the tensor-core path, 0 if the caller should use the FFMA kernel, < 0 on error
 int gemm_nt_f32_tc(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t lda, int64_t a_bs, const float* B,
                    int64_t ldb, int64_t b_bs, float beta, float* C, int64_t ldc, int64_t c_bs, int32_t lower,
                    int32_t batch, cudaStream_t stream) {
@@ -254,8 +238,7 @@ int convert_panel_f32(const double* P, int64_t ldp, int64_t rows, int64_t K, flo
   if (total == 0) return 0;
   f64_to_f32_panel_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(P, ldp, ws, rows, K);
   GPK_COUNT_LAUNCH();
-  cudaError_t e = cudaGetLastError();
-  return e == cudaSuccess ? 0 : -1000 - (int)e;
+  return cuda_rc(cudaGetLastError());
 }
 
 }  // namespace gpk

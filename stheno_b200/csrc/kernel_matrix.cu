@@ -36,27 +36,6 @@ struct KmParams {
   int64_t rows_out, cols_out;
 };
 
-template <typename T>
-__device__ __forceinline__ T t_exp(T v);
-template <>
-__device__ __forceinline__ double t_exp<double>(double v) {
-  return exp(v);
-}
-template <>
-__device__ __forceinline__ float t_exp<float>(float v) {
-  return expf(v);
-}
-template <typename T>
-__device__ __forceinline__ T t_sqrt(T v);
-template <>
-__device__ __forceinline__ double t_sqrt<double>(double v) {
-  return sqrt(v);
-}
-template <>
-__device__ __forceinline__ float t_sqrt<float>(float v) {
-  return sqrtf(v);
-}
-
 // phi(kind) from squared distance d2 / dot product.  d == 1 mirrors lab's |x - y| special case (no 1e-30 clamp).
 template <typename T>
 __device__ __forceinline__ T eval_factor(int kind, T d2, T dot, bool same_point, bool same_obj, int d, double param = 0.0) {
@@ -551,6 +530,17 @@ static int launch_kernel_matrix(const gpk_kernel_desc* desc, const T* xg, int64_
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();
   return 0;
+}
+
+int kernel_rows(const gpk_kernel_desc* desc, const double* xg, int64_t xg_gstride, int64_t n, const double* yg,
+                int64_t yg_gstride, int64_t n2, int32_t d, double* out, int64_t ldo, cudaStream_t stream) {
+  return launch_kernel_matrix<double>(desc, xg, xg_gstride, 0, n, yg, yg_gstride, 0, n2, d, 0.0, nullptr, 0, 0.0,
+                                      GPK_KM_PAD_ZERO, out, ldo, 0, 1, stream);
+}
+int kernel_rows(const gpk_kernel_desc* desc, const float* xg, int64_t xg_gstride, int64_t n, const float* yg,
+                int64_t yg_gstride, int64_t n2, int32_t d, float* out, int64_t ldo, cudaStream_t stream) {
+  return launch_kernel_matrix<float>(desc, xg, xg_gstride, 0, n, yg, yg_gstride, 0, n2, d, 0.0, nullptr, 0, 0.0,
+                                     GPK_KM_PAD_ZERO, out, ldo, 0, 1, stream);
 }
 
 // ---- elwise ------------------------------------------------------------------------------------------

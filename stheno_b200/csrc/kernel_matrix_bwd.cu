@@ -37,15 +37,6 @@ struct KbParams {
   void* param_sum; // [batch][GPK_MAX_FACTORS] or NULL
 };
 
-template <typename T>
-__device__ __forceinline__ T kb_exp(T v) {
-  return sizeof(T) == 8 ? (T)exp((double)v) : (T)expf((float)v);
-}
-template <typename T>
-__device__ __forceinline__ T kb_sqrt(T v) {
-  return sizeof(T) == 8 ? (T)sqrt((double)v) : (T)sqrtf((float)v);
-}
-
 // h(w) = log1p(w) - w / (1 + w) >= 0: d/da (1 + w)^-a = -(1 + w)^-a h(w) at fixed d2 (w = d2 / (2 a)).  The direct form
 // cancels for small w (h ~ w^2 / 2).  With s = w / (2 + w), -log1p(-t) = 2 atanh(s) for t = w / (1 + w) = 2 s / (1 + s), so
 //   h = 2 atanh(s) - t = 2 s^2 / (1 + s) + 2 s^3 sum_{j>=0} s^2j / (2j + 3),
@@ -90,7 +81,7 @@ __device__ __forceinline__ void eval_factor_grad(int kind, T d2, T dot, bool sam
       return;
     }
     case GPK_EQ: {
-      val = kb_exp<T>(T(-0.5) * d2);
+      val = t_exp<T>(T(-0.5) * d2);
       dval = T(-0.5) * val;
       return;
     }
@@ -98,23 +89,23 @@ __device__ __forceinline__ void eval_factor_grad(int kind, T d2, T dot, bool sam
       // not differentiable at r = 0: coincident points get the subgradient 0, the value autograd gives through the
       // reference's |x - y| (d = 1) and sqrt(max(d2, 1e-30)) (d > 1)
       const bool flat = (d == 1) ? !(d2 > T(0)) : !(d2 > T(1e-30));
-      T r = (d == 1) ? kb_sqrt<T>(d2) : kb_sqrt<T>(d2 > T(1e-30) ? d2 : T(1e-30));
-      val = kb_exp<T>(-r);
+      T r = (d == 1) ? t_sqrt<T>(d2) : t_sqrt<T>(d2 > T(1e-30) ? d2 : T(1e-30));
+      val = t_exp<T>(-r);
       dval = (same_pt || flat) ? T(0) : -val / (T(2) * r);
       return;
     }
     case GPK_MATERN32: {
-      T r = (d == 1) ? kb_sqrt<T>(d2) : kb_sqrt<T>(d2 > T(1e-30) ? d2 : T(1e-30));
+      T r = (d == 1) ? t_sqrt<T>(d2) : t_sqrt<T>(d2 > T(1e-30) ? d2 : T(1e-30));
       T s = T(1.7320508075688772) * r;
-      T e = kb_exp<T>(-s);
+      T e = t_exp<T>(-s);
       val = (T(1) + s) * e;
       dval = T(-1.5) * e;
       return;
     }
     case GPK_MATERN52: {
-      T r = (d == 1) ? kb_sqrt<T>(d2) : kb_sqrt<T>(d2 > T(1e-30) ? d2 : T(1e-30));
+      T r = (d == 1) ? t_sqrt<T>(d2) : t_sqrt<T>(d2 > T(1e-30) ? d2 : T(1e-30));
       T s = T(2.23606797749979) * r;
-      T e = kb_exp<T>(-s);
+      T e = t_exp<T>(-s);
       val = (T(1) + s + T(1.6666666666666667) * d2) * e;
       dval = T(-0.8333333333333334) * (T(1) + s) * e;
       return;

@@ -18,37 +18,6 @@
 namespace gpk {
 
 template <typename T>
-struct PostAbi;
-template <>
-struct PostAbi<double> {
-  static int km(const gpk_kernel_desc* d, const double* x, int64_t xg, int64_t n, const double* y, int64_t yg, int64_t n2, int32_t dim,
-                double* out, int64_t ldo, void* s) {
-    return gpk_kernel_matrix_f64(d, x, xg, 0, n, y, yg, 0, n2, dim, 0.0, nullptr, 0, 0.0, GPK_KM_PAD_ZERO, out, ldo, 0, 1, s);
-  }
-  static int trsm(const double* L, int64_t ldl, int64_t n, double* B, int64_t ldb, int64_t rows, int32_t S, void* ws,
-                  int64_t ws_bytes, void* s) {
-    return gpk_trsm_right_f64(L, ldl, 0, n, B, ldb, 0, rows, 1, S, ws, ws_bytes, s);
-  }
-  static int red(const double* V, int64_t ldv, int64_t rows, int64_t nc, const double* b, double* dot, double* sq, void* s) {
-    return gpk_row_dot_sq_f64(V, ldv, 0, rows, nc, b, 0, dot, sq, 0, 1, s);
-  }
-};
-template <>
-struct PostAbi<float> {
-  static int km(const gpk_kernel_desc* d, const float* x, int64_t xg, int64_t n, const float* y, int64_t yg, int64_t n2, int32_t dim,
-                float* out, int64_t ldo, void* s) {
-    return gpk_kernel_matrix_f32(d, x, xg, 0, n, y, yg, 0, n2, dim, 0.0, nullptr, 0, 0.0, GPK_KM_PAD_ZERO, out, ldo, 0, 1, s);
-  }
-  static int trsm(const float* L, int64_t ldl, int64_t n, float* B, int64_t ldb, int64_t rows, int32_t, void*, int64_t,
-                  void* s) {
-    return gpk_trsm_right_f32(L, ldl, 0, n, B, ldb, 0, rows, 1, s);
-  }
-  static int red(const float* V, int64_t ldv, int64_t rows, int64_t nc, const float* b, float* dot, float* sq, void* s) {
-    return gpk_row_dot_sq_f32(V, ldv, 0, rows, nc, b, 0, dot, sq, 0, 1, s);
-  }
-};
-
-template <typename T>
 static int posterior_marginals(const gpk_kernel_desc* desc, const T* xsg, int64_t xsg_gstride, int64_t m, const T* xg,
                                int64_t xg_gstride, int64_t n, int32_t d, const T* L, int64_t ldl, int64_t n_pad,
                                const T* half_y, T* dot, T* sq, int64_t chunk, T* ws, int64_t ws_elems, int32_t slices,
@@ -58,13 +27,14 @@ static int posterior_marginals(const gpk_kernel_desc* desc, const T* xsg, int64_
   if (ws_elems < chunk * n_pad || reinterpret_cast<uintptr_t>(ws) % 16) return GPK_ERR_ARG;
   if (!dot && !sq) return GPK_ERR_ARG;
   if (dot && !half_y) return GPK_ERR_ARG;
+  cudaStream_t s = (cudaStream_t)stream;
   int rc;
   for (int64_t a = 0; a < m; a += chunk) {
     const int64_t c = (m - a < chunk) ? m - a : chunk;
     const int64_t c_pad = (c + 127) / 128 * 128;
-    if ((rc = PostAbi<T>::km(desc, xsg + a * d, xsg_gstride, c, xg, xg_gstride, n, d, ws, n_pad, stream))) return rc;
-    if ((rc = PostAbi<T>::trsm(L, ldl, n_pad, ws, n_pad, c_pad, slices, oz_ws, oz_ws_bytes, stream))) return rc;
-    if ((rc = PostAbi<T>::red(ws, n_pad, c, n_pad, half_y, dot ? dot + a : nullptr, sq ? sq + a : nullptr, stream))) return rc;
+    if ((rc = kernel_rows(desc, xsg + a * d, xsg_gstride, c, xg, xg_gstride, n, d, ws, n_pad, s))) return rc;
+    if ((rc = trsm_right(L, ldl, n_pad, ws, n_pad, c_pad, slices, oz_ws, oz_ws_bytes, s))) return rc;
+    if ((rc = row_dot_sq(ws, n_pad, c, n_pad, half_y, dot ? dot + a : nullptr, sq ? sq + a : nullptr, s))) return rc;
   }
   return 0;
 }
@@ -118,11 +88,10 @@ static int sparse_posterior_marginals(const gpk_kernel_desc* desc, const T* xsg,
   for (int64_t a = 0; a < ns; a += chunk) {
     const int64_t c = (ns - a < chunk) ? ns - a : chunk;
     const int64_t c_pad = (c + 127) / 128 * 128;
-    if ((rc = PostAbi<T>::km(desc, xsg + a * d, xsg_gstride, c, zg, zg_gstride, m, d, V, m_pad, stream))) return rc;
-    const cudaError_t e = cudaMemcpyAsync(U, V, (size_t)(c_pad * m_pad) * sizeof(T), cudaMemcpyDeviceToDevice, s);
-    if (e != cudaSuccess) return -1000 - (int)e;
-    if ((rc = PostAbi<T>::trsm(Lz, ldlz, m_pad, V, m_pad, c_pad, slices, oz_ws, oz_ws_bytes, stream))) return rc;
-    if ((rc = PostAbi<T>::trsm(LS, ldls, m_pad, U, m_pad, c_pad, slices, oz_ws, oz_ws_bytes, stream))) return rc;
+    if ((rc = kernel_rows(desc, xsg + a * d, xsg_gstride, c, zg, zg_gstride, m, d, V, m_pad, s))) return rc;
+    if ((rc = cuda_rc(cudaMemcpyAsync(U, V, (size_t)(c_pad * m_pad) * sizeof(T), cudaMemcpyDeviceToDevice, s)))) return rc;
+    if ((rc = trsm_right(Lz, ldlz, m_pad, V, m_pad, c_pad, slices, oz_ws, oz_ws_bytes, s))) return rc;
+    if ((rc = trsm_right(LS, ldls, m_pad, U, m_pad, c_pad, slices, oz_ws, oz_ws_bytes, s))) return rc;
     sparse_post_rows_kernel<T><<<(unsigned)(c_pad / 8), 256, 0, s>>>(c, m_pad, V, U, m_pad, half_y, dot ? dot + a : nullptr,
                                                                     sq_z + a, sq_s + a);
     GPK_COUNT_LAUNCH();

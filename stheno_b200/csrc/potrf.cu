@@ -29,37 +29,7 @@
 
 namespace gpk {
 
-int gemm_nt_f64(int64_t, int64_t, int64_t, double, const double*, int64_t, int64_t, const double*, int64_t, int64_t,
-                double, double*, int64_t, int64_t, int32_t, int32_t, int32_t, void*, int64_t, cudaStream_t);
-int gemm_nt_f32(int64_t, int64_t, int64_t, float, const float*, int64_t, int64_t, const float*, int64_t, int64_t,
-                float, float*, int64_t, int64_t, int32_t, int32_t, cudaStream_t);
-
-// (S, ws, ws_bytes): the int8-slice emulation the caller asked for (gpk.h); fp32 has none
-static inline int gemm_nt(int64_t M, int64_t N, int64_t K, double alpha, const double* A, int64_t lda, int64_t a_bs,
-                          const double* B, int64_t ldb, int64_t b_bs, double beta, double* C, int64_t ldc, int64_t c_bs,
-                          int32_t lower, int32_t batch, int32_t S, void* ws, int64_t ws_bytes, cudaStream_t s) {
-  return gemm_nt_f64(M, N, K, alpha, A, lda, a_bs, B, ldb, b_bs, beta, C, ldc, c_bs, lower, batch, S, ws, ws_bytes, s);
-}
-static inline int gemm_nt(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t lda, int64_t a_bs,
-                          const float* B, int64_t ldb, int64_t b_bs, float beta, float* C, int64_t ldc, int64_t c_bs,
-                          int32_t lower, int32_t batch, int32_t, void*, int64_t, cudaStream_t s) {
-  return gemm_nt_f32(M, N, K, alpha, A, lda, a_bs, B, ldb, b_bs, beta, C, ldc, c_bs, lower, batch, s);
-}
-
 constexpr int NB = 128;
-
-template <typename T>
-__device__ __forceinline__ T t_sqrt_(T v) {
-  return sizeof(T) == 8 ? (T)sqrt((double)v) : (T)sqrtf((float)v);
-}
-template <typename T>
-__device__ __forceinline__ T t_rsqrt_(T v) {
-  return sizeof(T) == 8 ? (T)rsqrt((double)v) : (T)rsqrtf((float)v);
-}
-template <typename T>
-__device__ __forceinline__ T t_log_(T v) {
-  return sizeof(T) == 8 ? (T)log((double)v) : (T)logf((float)v);
-}
 
 // ---- leaf Cholesky: 128 x 128 block in registers ----------------------------------------------------------
 // thread (ti, tk) = (tid / 16, tid % 16) owns elements (i, k) = (ti + 16 a, tk + 16 b), a, b < 8.
@@ -94,7 +64,7 @@ potrf_leaf_kernel(T* __restrict__ A, int64_t lda, int64_t a_bs, T* __restrict__ 
       if (tid == 0 && !(djj > T(0))) atomicCAS(info + bidx, 0, pivot_base + j + 1);
       // 1/sqrt via the hardware reciprocal-sqrt seed (+ Newton steps, <= 1 ulp) and sqrt = d * rsqrt(d): takes the
       // IEEE sqrt + divide software sequences (~350 cycles in fp64) off the per-column critical path.
-      const T inv = t_rsqrt_<T>(djj);
+      const T inv = t_rsqrt<T>(djj);
       const T dsq = djj * inv;
       T li[8], lk[8];
 #pragma unroll
@@ -135,7 +105,7 @@ potrf_leaf_kernel(T* __restrict__ A, int64_t lda, int64_t a_bs, T* __restrict__ 
 
   __syncthreads();
   if (logdet != nullptr) {
-    T v = (tid < NB) ? t_log_<T>(diag[tid]) : T(0);
+    T v = (tid < NB) ? t_log<T>(diag[tid]) : T(0);
     v = warp_sum(v);
     if ((tid & 31) == 0) red[tid >> 5] = v;
     __syncthreads();
@@ -350,16 +320,15 @@ potrf_leaf_rec_kernel(T* __restrict__ A, int64_t lda, int64_t a_bs, T* __restric
   if (dbg) dbg[dbg_i++] = clock64();
 }
 
-// ---- leaf TRSM:  X L^T = B  (B: rows x 128, 64 rows per CTA), in place ----------------------------------------
-// thread (r, cg) = (tid % 64, tid / 64) owns row r, columns 32 cg .. 32 cg + 31 in registers.
-// UPPER == true solves X L = B instead (backward substitution; L still lower-triangular).
+// ---- leaf TRSM of gpk_trsm_right_t:  X L = B  (B: rows x 128, 64 rows per CTA), in place, by backward substitution
+// (L lower-triangular).  Thread (r, cg) = (tid % 64, tid / 64) owns row r, columns 32 cg .. 32 cg + 31 in registers.
 constexpr int TL_LD = NB + 2;
 
-template <typename T, bool TRANS>
+template <typename T>
 __global__ void __launch_bounds__(256, 1)
 trsm_leaf_kernel(const T* __restrict__ L, int64_t ldl, int64_t l_bs, T* __restrict__ B, int64_t ldb, int64_t b_bs) {
   extern __shared__ __align__(16) unsigned char tl_smem[];
-  T* Lt = reinterpret_cast<T*>(tl_smem);  // !TRANS: Lt[j][k] = L[k][j];  TRANS: Lt[j][k] = L[j][k]   (ld = TL_LD)
+  T* Lt = reinterpret_cast<T*>(tl_smem);  // Lt[j][k] = L[j][k]   (ld = TL_LD)
   T* invd = Lt + NB * TL_LD;              // 1 / L[j][j]
   T* xbuf = invd + NB;                    // [2][64]
   const int tid = threadIdx.x;
@@ -370,8 +339,7 @@ trsm_leaf_kernel(const T* __restrict__ L, int64_t ldl, int64_t l_bs, T* __restri
   for (int idx = tid; idx < NB * NB; idx += 256) {
     const int k = idx >> 7, j = idx & 127;  // read L[k][j] coalesced in j
     const T v = (j <= k) ? L[(int64_t)k * ldl + j] : T(0);
-    if (!TRANS) Lt[j * TL_LD + k] = v;
-    else Lt[k * TL_LD + j] = v;
+    Lt[k * TL_LD + j] = v;
     if (j == k) invd[j] = T(1) / v;
   }
   const int r = tid & 63, cg = tid >> 6;
@@ -385,8 +353,7 @@ trsm_leaf_kernel(const T* __restrict__ L, int64_t ldl, int64_t l_bs, T* __restri
 
   int buf = 0;
   for (int step = 0; step < NB; ++step) {
-    // forward: j = 0..127 ; backward (TRANS): j = 127..0
-    const int j = TRANS ? (NB - 1 - step) : step;
+    const int j = NB - 1 - step;
     const int cgj = j >> 5, jj = j & 31;
     if (cg == cgj) {
       T x = T(0);
@@ -398,14 +365,13 @@ trsm_leaf_kernel(const T* __restrict__ L, int64_t ldl, int64_t l_bs, T* __restri
       xbuf[buf * 64 + r] = x;
     }
     __syncthreads();
-    const bool active = TRANS ? (cg <= cgj) : (cg >= cgj);
-    if (active) {
+    if (cg <= cgj) {
       const T x = xbuf[buf * 64 + r];
-      // !TRANS: a[k] -= x * L[k][j] (k > j) = Lt[j][k];  TRANS: a[k] -= x * L[j][k] (k < j) = Lt[j][k]
+      // a[k] -= x * L[j][k] (k < j) = Lt[j][k]
       const T* lrow = Lt + j * TL_LD + 32 * cg;
 #pragma unroll
       for (int q = 0; q < 32; ++q) {
-        const bool ok = (cg != cgj) || (TRANS ? (q < jj) : (q > jj));
+        const bool ok = (cg != cgj) || (q < jj);
         if (ok) a[q] -= x * lrow[q];
       }
     }
@@ -543,9 +509,11 @@ trsm_leaf_tc_kernel(const T* __restrict__ L, int64_t ldl, int64_t l_bs, T* __res
   }
 }
 
+// X L^T = B against a 128 x 128 leaf L, 128 rows of B per CTA: rows must be a multiple of 128
 template <typename T>
-static int launch_trsm_leaf_tc(const T* L, int64_t ldl, int64_t l_bs, T* B, int64_t ldb, int64_t b_bs, int64_t rows,
-                               int32_t batch, cudaStream_t stream) {
+static int trsm_leaf_fwd(const T* L, int64_t ldl, int64_t l_bs, T* B, int64_t ldb, int64_t b_bs, int64_t rows,
+                         int32_t batch, cudaStream_t stream) {
+  if (rows % TC_ROWS) return GPK_ERR_ARG;
   if (rows == 0) return 0;
   if (const int rc = opt_in_smem<trsm_leaf_tc_kernel<T>>(TC_SMEM)) return rc;
   dim3 grid((unsigned)(rows / TC_ROWS), (unsigned)batch);
@@ -629,24 +597,17 @@ static int launch_potrf_leaf(T* A, int64_t lda, int64_t a_bs, T* logdet, int32_t
   return 0;
 }
 
-template <typename T, bool TRANS>
+template <typename T>
 static int launch_trsm_leaf(const T* L, int64_t ldl, int64_t l_bs, T* B, int64_t ldb, int64_t b_bs, int64_t rows,
                             int32_t batch, cudaStream_t stream) {
   if (rows == 0) return 0;
   const int smem = (NB * TL_LD + NB + 2 * 64) * (int)sizeof(T);
-  if (const int rc = opt_in_smem<trsm_leaf_kernel<T, TRANS>>(smem)) return rc;
+  if (const int rc = opt_in_smem<trsm_leaf_kernel<T>>(smem)) return rc;
   dim3 grid((unsigned)(rows / 64), (unsigned)batch);
-  trsm_leaf_kernel<T, TRANS><<<grid, 256, smem, stream>>>(L, ldl, l_bs, B, ldb, b_bs);
+  trsm_leaf_kernel<T><<<grid, 256, smem, stream>>>(L, ldl, l_bs, B, ldb, b_bs);
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();
   return 0;
-}
-
-template <typename T>
-static int trsm_leaf_fwd(const T* L, int64_t ldl, int64_t l_bs, T* B, int64_t ldb, int64_t b_bs, int64_t rows,
-                         int32_t batch, cudaStream_t stream) {
-  if (rows % TC_ROWS == 0) return launch_trsm_leaf_tc<T>(L, ldl, l_bs, B, ldb, b_bs, rows, batch, stream);
-  return launch_trsm_leaf<T, false>(L, ldl, l_bs, B, ldb, b_bs, rows, batch, stream);
 }
 
 constexpr int64_t NB_OUTER = 512;  // outer panel width
@@ -717,7 +678,6 @@ static int factor_panel(T* A, int64_t lda, int64_t a_bs, int64_t R, int64_t kb, 
 template <typename T>
 static int factor_panel_split(T* A, int64_t lda, int64_t a_bs, int64_t R, int64_t kb, int64_t ke, T* logdet, int32_t* info,
                               int32_t batch, cudaStream_t chain, Lookahead& la) {
-  auto ce = [](cudaError_t e) { return e == cudaSuccess ? 0 : -1000 - (int)e; };
   int rc;
   bool bulk_pending = false;  // bulk work the next diag_step has to wait for
   for (int64_t j = kb; j < ke; j += NB) {
@@ -728,31 +688,31 @@ static int factor_panel_split(T* A, int64_t lda, int64_t a_bs, int64_t R, int64_
     const int64_t b0 = has_next ? j1 + NB : j1;  // first row the bulk stream handles
     const int64_t brows = R - b0;
     if (brows > 0) {
-      if ((rc = ce(cudaEventRecord(la.leaf, chain)))) return rc;
-      if ((rc = ce(cudaStreamWaitEvent(la.bulk, la.leaf, 0)))) return rc;
+      if ((rc = cuda_rc(cudaEventRecord(la.leaf, chain)))) return rc;
+      if ((rc = cuda_rc(cudaStreamWaitEvent(la.bulk, la.leaf, 0)))) return rc;
       if ((rc = trsm_leaf_fwd<T>(Ajj, lda, a_bs, A + b0 * lda + j, lda, a_bs, brows, batch, la.bulk))) return rc;
     }
     if (has_next) {
       if (bulk_pending) {  // the rows this step solves were updated by the previous step's bulk GEMM
-        if ((rc = ce(cudaStreamWaitEvent(chain, la.bulk_done, 0)))) return rc;
+        if ((rc = cuda_rc(cudaStreamWaitEvent(chain, la.bulk_done, 0)))) return rc;
       }
       T* X1 = A + j1 * lda + j;  // rows [j1, j1 + 128) of this block column
       if ((rc = launch_diag_step<T>(Ajj, lda, a_bs, X1, lda, a_bs, A + j1 * lda + j1, lda, a_bs, batch, chain))) return rc;
       if (brows > 0) {
-        if ((rc = ce(cudaEventRecord(la.crit, chain)))) return rc;
-        if ((rc = ce(cudaStreamWaitEvent(la.bulk, la.crit, 0)))) return rc;
+        if ((rc = cuda_rc(cudaEventRecord(la.crit, chain)))) return rc;
+        if ((rc = cuda_rc(cudaStreamWaitEvent(la.bulk, la.crit, 0)))) return rc;
         // rows [b0, R) x columns [j1, ke) of the panel -= X[b0:, j] X[j1:ke, j]^T
         if ((rc = gemm_nt(brows, ke - j1, (int64_t)NB, T(-1), A + b0 * lda + j, lda, a_bs, X1, lda, a_bs, T(1),
                           A + b0 * lda + j1, lda, a_bs, 0, batch, 0, nullptr, 0, la.bulk)))
           return rc;
-        if ((rc = ce(cudaEventRecord(la.bulk_done, la.bulk)))) return rc;
+        if ((rc = cuda_rc(cudaEventRecord(la.bulk_done, la.bulk)))) return rc;
         bulk_pending = true;
       }
     }
   }
   if (R - ke > 0 || bulk_pending) {
-    if ((rc = ce(cudaEventRecord(la.bulk_done, la.bulk)))) return rc;
-    if ((rc = ce(cudaStreamWaitEvent(chain, la.bulk_done, 0)))) return rc;
+    if ((rc = cuda_rc(cudaEventRecord(la.bulk_done, la.bulk)))) return rc;
+    if ((rc = cuda_rc(cudaStreamWaitEvent(chain, la.bulk_done, 0)))) return rc;
   }
   return 0;
 }
@@ -761,12 +721,6 @@ static int factor_panel_split(T* A, int64_t lda, int64_t a_bs, int64_t R, int64_
 // (a) the columns of panel i+1 and (b) everything to the right of it; as soon as (a) is done the latency-bound
 // factorisation of panel i+1 runs on a high-priority side stream while the tensor-core-bound update (b) keeps the
 // SMs busy on the caller's stream.
-int syrk_f64_tf32x3(int64_t, int64_t, int64_t, const float*, double*, int64_t, cudaStream_t);  // gemm_tc32.cu
-int convert_panel_f32(const double*, int64_t, int64_t, int64_t, float*, cudaStream_t);
-int64_t oz_ws_bytes(int64_t rows, int64_t K, int32_t S);  // gemm_oz.cu
-int oz_slice_panel(const double*, int64_t, int64_t, int64_t, void*, int64_t, int32_t, cudaStream_t);
-int oz_gemm_sliced(int64_t, int64_t, int64_t, double, const void*, int64_t, int64_t, const void*, int64_t, int64_t, double,
-                   double*, int64_t, int32_t, int32_t, cudaStream_t);
 
 // How the K = NB_OUTER trailing updates of an fp64 factorisation are formed:
 //   MODE_F64     fp64 tensor cores (DMMA) straight from the matrix
@@ -842,7 +796,6 @@ int trailing_update<double>(int used, const Trailing& t, int64_t rA, int64_t rB,
 // Updates that touch the same block are ordered by streams / events (never concurrent: results stay bit-reproducible).
 static int potrf_driver_pairs(double* A, int64_t lda, int64_t n_pad, int64_t extra_rows, double* logdet, int32_t* info,
                               cudaStream_t stream, void* ws, int32_t S, Lookahead& la) {
-  auto ce = [](cudaError_t e) { return e == cudaSuccess ? 0 : -1000 - (int)e; };
   const int64_t R = n_pad + extra_rows, P = NB_OUTER;
   const bool nola = no_lookahead();  // the same schedule on ONE stream
   const cudaStream_t side = nola ? stream : la.side, bulk = nola ? stream : la.bulk;
@@ -872,9 +825,9 @@ static int potrf_driver_pairs(double* A, int64_t lda, int64_t n_pad, int64_t ext
     const int64_t ke2 = ke + 2 * P < n_pad ? ke + 2 * P : n_pad;      // B' = [ke1, ke2) (may be empty)
     const int64_t W1 = ke1 - ke, W2 = ke2 - ke1, K2 = 2 * P;
     if ((rc = oz_slice_panel(A + ke * lda + kb, lda, R - ke, K2, wsX, R, S, stream))) return rc;
-    if ((rc = ce(cudaEventRecord(la.fork, stream)))) return rc;
-    if ((rc = ce(cudaStreamWaitEvent(side, la.fork, 0)))) return rc;
-    if ((rc = ce(cudaStreamWaitEvent(bulk, la.fork, 0)))) return rc;
+    if ((rc = cuda_rc(cudaEventRecord(la.fork, stream)))) return rc;
+    if ((rc = cuda_rc(cudaStreamWaitEvent(side, la.fork, 0)))) return rc;
+    if ((rc = cuda_rc(cudaStreamWaitEvent(bulk, la.fork, 0)))) return rc;
     // block column A': its diagonal block on the chain stream (the leaf chain starts on it at once), the rows below on bulk
     if ((rc = upd(wsX, K2, 0, 0, W1, W1, A + ke * lda + ke, 1, side))) return rc;
     if ((rc = upd(wsX, K2, W1, 0, R - ke1, W1, A + ke1 * lda + ke, 0, bulk))) return rc;
@@ -884,15 +837,15 @@ static int potrf_driver_pairs(double* A, int64_t lda, int64_t n_pad, int64_t ext
     if (W2 > 0) {
       if ((rc = oz_slice_panel(A + ke1 * lda + ke, lda, R - ke1, W1, wsY, R, S, side))) return rc;
       if ((rc = upd(wsY, W1, 0, 0, W2, W2, A + ke1 * lda + ke1, 1, side))) return rc;
-      if ((rc = ce(cudaEventRecord(la.crit, side)))) return rc;  // Y is ready (and every earlier update of B' is done)
-      if ((rc = ce(cudaStreamWaitEvent(bulk, la.crit, 0)))) return rc;
+      if ((rc = cuda_rc(cudaEventRecord(la.crit, side)))) return rc;  // Y is ready (and every earlier update of B' is done)
+      if ((rc = cuda_rc(cudaStreamWaitEvent(bulk, la.crit, 0)))) return rc;
       if ((rc = upd(wsY, W1, W2, 0, R - ke2, W2, A + ke2 * lda + ke1, 0, bulk))) return rc;
       if ((rc = factor(ke1, ke2))) return rc;
     }
-    if ((rc = ce(cudaEventRecord(la.join, side)))) return rc;
+    if ((rc = cuda_rc(cudaEventRecord(la.join, side)))) return rc;
     // the far part: everything right of the next pair, K = 1024, on the caller's stream
     if ((rc = upd(wsX, K2, ke2 - ke, ke2 - ke, R - ke2, n_pad - ke2, A + ke2 * lda + ke2, 1, stream))) return rc;
-    if ((rc = ce(cudaStreamWaitEvent(stream, la.join, 0)))) return rc;
+    if ((rc = cuda_rc(cudaStreamWaitEvent(stream, la.join, 0)))) return rc;
   }
   return 0;
 }
@@ -912,7 +865,6 @@ static int potrf_driver(T* A, int64_t lda, int64_t a_bs, int64_t n_pad, int64_t 
     return potrf_driver_pairs(reinterpret_cast<double*>(A), lda, n_pad, extra_rows, reinterpret_cast<double*>(logdet), info,
                               stream, tr.ws, tr.slices, la);
   const bool use_la = la.ok && n_pad > 2 * NB_OUTER && !no_lookahead();
-  auto ce = [](cudaError_t e) { return e == cudaSuccess ? 0 : -1000 - (int)e; };
 
   const int64_t ke0 = NB_OUTER < n_pad ? NB_OUTER : n_pad;
   if ((rc = factor_panel<T>(A, lda, a_bs, R, 0, ke0, logdet, info, batch, stream))) return rc;
@@ -932,25 +884,25 @@ static int potrf_driver(T* A, int64_t lda, int64_t a_bs, int64_t n_pad, int64_t 
       // side streams (high priority): (a) the next panel's columns, then that panel's factorisation;
       // caller's stream: (b) everything to the right of it.  (a) and (b) are independent (both only read panel i), so
       // they run concurrently and the short (a) no longer costs a kernel tail of its own.
-      if ((rc = ce(cudaEventRecord(la.fork, stream)))) return rc;
-      if ((rc = ce(cudaStreamWaitEvent(la.side, la.fork, 0)))) return rc;
+      if ((rc = cuda_rc(cudaEventRecord(la.fork, stream)))) return rc;
+      if ((rc = cuda_rc(cudaStreamWaitEvent(la.side, la.fork, 0)))) return rc;
       if (used != MODE_TF32X3) {
         // (a) in two parts: the next panel's diagonal block first (the chain starts on it at once), the rows below on `bulk`
-        if ((rc = ce(cudaStreamWaitEvent(la.bulk, la.fork, 0)))) return rc;
+        if ((rc = cuda_rc(cudaStreamWaitEvent(la.bulk, la.fork, 0)))) return rc;
         if ((rc = trailing_update<T>(used, tr, 0, 0, W, W, K, P, P, lda, a_bs, Ckk, 1, batch, la.side))) return rc;
         if (R - ke2 > 0 && (rc = trailing_update<T>(used, tr, W, 0, R - ke2, W, K, P2, P, lda, a_bs, A + ke2 * lda + ke, 0,
                                                     batch, la.bulk)))
           return rc;
       } else {
         if ((rc = trailing_update<T>(used, tr, 0, 0, R - ke, W, K, P, P, lda, a_bs, Ckk, 1, batch, la.side))) return rc;
-        if ((rc = ce(cudaStreamWaitEvent(la.bulk, la.fork, 0)))) return rc;
+        if ((rc = cuda_rc(cudaStreamWaitEvent(la.bulk, la.fork, 0)))) return rc;
       }
       if ((rc = factor_panel_split<T>(A, lda, a_bs, R, ke, ke2, logdet, info, batch, la.side, la))) return rc;
-      if ((rc = ce(cudaEventRecord(la.join, la.side)))) return rc;
+      if ((rc = cuda_rc(cudaEventRecord(la.join, la.side)))) return rc;
       if ((rc = trailing_update<T>(used, tr, W, W, R - ke2, n_pad - ke2, K, P2, P2, lda, a_bs, A + ke2 * lda + ke2, 1, batch,
                                    stream)))
         return rc;
-      if ((rc = ce(cudaStreamWaitEvent(stream, la.join, 0)))) return rc;
+      if ((rc = cuda_rc(cudaStreamWaitEvent(stream, la.join, 0)))) return rc;
     } else {
       if ((rc = trailing_update<T>(used, tr, 0, 0, R - ke, W, K, P, P, lda, a_bs, Ckk, 1, batch, stream))) return rc;
       if (more) {
@@ -993,6 +945,15 @@ static int trsm_right_driver(const T* L, int64_t ldl, int64_t l_bs, int64_t n_pa
   return trsm_right_rec<T>(L, ldl, l_bs, n_pad, B, ldb, b_bs, rows, batch, S, ws, ws_bytes, stream);
 }
 
+int trsm_right(const double* L, int64_t ldl, int64_t n_pad, double* B, int64_t ldb, int64_t rows, int32_t S, void* ws,
+               int64_t ws_bytes, cudaStream_t stream) {
+  return trsm_right_driver<double>(L, ldl, 0, n_pad, B, ldb, 0, rows, 1, S, ws, ws_bytes, stream);
+}
+int trsm_right(const float* L, int64_t ldl, int64_t n_pad, float* B, int64_t ldb, int64_t rows, int32_t, void*, int64_t,
+               cudaStream_t stream) {
+  return trsm_right_driver<float>(L, ldl, 0, n_pad, B, ldb, 0, rows, 1, 0, nullptr, 0, stream);
+}
+
 // X L = B (backward substitution), right-looking over 128-blocks from the last to the first.  The off-diagonal
 // update  B[:, 0:j] -= X_j L[j, 0:j]  is a rank-128 "NN" product; it is expressed with gemm_nt through an explicit
 // transposed copy of the L row-panel made by the caller-provided scratch -- used only for few right-hand sides
@@ -1024,7 +985,7 @@ static int trsm_right_t_driver(const T* L, int64_t ldl, int64_t l_bs, int64_t n_
   if (rows == 0) return 0;
   int rc;
   for (int64_t j = n_pad - NB; j >= 0; j -= NB) {
-    if ((rc = launch_trsm_leaf<T, true>(L + j * ldl + j, ldl, l_bs, B + j, ldb, b_bs, rows, batch, stream))) return rc;
+    if ((rc = launch_trsm_leaf<T>(L + j * ldl + j, ldl, l_bs, B + j, ldb, b_bs, rows, batch, stream))) return rc;
     if (j > 0) {
       dim3 grid((unsigned)((j + 127) / 128), (unsigned)rows, (unsigned)batch);
       trsm_t_update_kernel<T><<<grid, 128, 0, stream>>>(L, ldl, l_bs, B, ldb, b_bs, j, rows);
@@ -1040,8 +1001,7 @@ static int trsm_right_t_driver(const T* L, int64_t ldl, int64_t l_bs, int64_t n_
 extern "C" {
 int gpk_debug_leaf_phase_clock(void* buf16_int64) {
   long long* p = static_cast<long long*>(buf16_int64);
-  cudaError_t e = cudaMemcpyToSymbol(gpk::g_leaf_phase_clock, &p, sizeof(p));
-  return e == cudaSuccess ? 0 : -1000 - (int)e;
+  return gpk::cuda_rc(cudaMemcpyToSymbol(gpk::g_leaf_phase_clock, &p, sizeof(p)));
 }
 int64_t gpk_potrf_oz_ws_bytes(int64_t n_pad, int64_t extra_rows, int32_t slices) {
   if (slices < 5 || slices > 8 || n_pad < 2048) return 0;

@@ -113,44 +113,6 @@ __global__ void row_dot_acc_kernel(const T* __restrict__ V, int64_t ldv, int64_t
   if (lane == 0) acc[r] += (T)s;
 }
 
-template <typename T>
-struct SparseAbi;
-template <>
-struct SparseAbi<double> {
-  static int km(const gpk_kernel_desc* d, const double* x, int64_t xg, int64_t n, const double* y, int64_t yg, int64_t n2, int32_t dim,
-                double* out, int64_t ldo, void* s) {
-    return gpk_kernel_matrix_f64(d, x, xg, 0, n, y, yg, 0, n2, dim, 0.0, nullptr, 0, 0.0, GPK_KM_PAD_ZERO, out, ldo, 0, 1, s);
-  }
-  static int trsm(const double* L, int64_t ldl, int64_t n, double* B, int64_t ldb, int64_t rows, int32_t S, void* ws,
-                  int64_t ws_bytes, void* s) {
-    return gpk_trsm_right_f64(L, ldl, 0, n, B, ldb, 0, rows, 1, S, ws, ws_bytes, s);
-  }
-  static int sq(const double* V, int64_t ldv, int64_t rows, int64_t nc, double* out, void* s) {
-    return gpk_row_dot_sq_f64(V, ldv, 0, rows, nc, nullptr, 0, nullptr, out, 0, 1, s);
-  }
-  static int syrk(int64_t M, int64_t K, const double* A, int64_t lda, double* C, int64_t ldc, int32_t S, void* ws,
-                  int64_t ws_bytes, void* s) {
-    return gpk_gemm_nt_f64(M, M, K, 1.0, A, lda, 0, A, lda, 0, 1.0, C, ldc, 0, 1, 1, S, ws, ws_bytes, s);
-  }
-};
-template <>
-struct SparseAbi<float> {
-  static int km(const gpk_kernel_desc* d, const float* x, int64_t xg, int64_t n, const float* y, int64_t yg, int64_t n2, int32_t dim,
-                float* out, int64_t ldo, void* s) {
-    return gpk_kernel_matrix_f32(d, x, xg, 0, n, y, yg, 0, n2, dim, 0.0, nullptr, 0, 0.0, GPK_KM_PAD_ZERO, out, ldo, 0, 1, s);
-  }
-  static int trsm(const float* L, int64_t ldl, int64_t n, float* B, int64_t ldb, int64_t rows, int32_t, void*, int64_t,
-                  void* s) {
-    return gpk_trsm_right_f32(L, ldl, 0, n, B, ldb, 0, rows, 1, s);
-  }
-  static int sq(const float* V, int64_t ldv, int64_t rows, int64_t nc, float* out, void* s) {
-    return gpk_row_dot_sq_f32(V, ldv, 0, rows, nc, nullptr, 0, nullptr, out, 0, 1, s);
-  }
-  static int syrk(int64_t M, int64_t K, const float* A, int64_t lda, float* C, int64_t ldc, int32_t, void*, int64_t, void* s) {
-    return gpk_gemm_nt_f32(M, M, K, 1.0f, A, lda, 0, A, lda, 0, 1.0f, C, ldc, 0, 1, 1, s);
-  }
-};
-
 // Backward of the streamed ELBO, per data point of a chunk (one warp per row; no atomics).  With s = A^-1 prod and the solved
 // rows w_i (Wc) and u_i = A^-1 w_i (U):  beta_i = s.w_i, gamma_i = w_i.u_i, r_i = ybar_i - beta_i, kappa_i = K_n' (:311-313),
 //   g_kappa = (r^2 + gamma - kappa) / (2 kappa^2),  dE/dybar_i = -r / kappa,
@@ -231,9 +193,9 @@ static int sparse_accumulate(const gpk_kernel_desc* desc, const T* xg, int64_t x
   double* partial = reinterpret_cast<double*>(ybs + c_pad);  // [3][nb]; 8-byte aligned: c_pad is a multiple of 128
   cudaStream_t s = (cudaStream_t)stream;
   int rc;
-  if ((rc = SparseAbi<T>::km(desc, xg, xg_gstride, c, zg, zg_gstride, m, d, Wc, m_pad, stream))) return rc;   // :285
-  if ((rc = SparseAbi<T>::trsm(Lz, ldl, m_pad, Wc, m_pad, c_pad, slices, oz_ws, oz_ws_bytes, stream))) return rc;                          // :301
-  if (method != 2 && (rc = SparseAbi<T>::sq(Wc, m_pad, c, m_pad, q, stream))) return rc;                       // :305
+  if ((rc = kernel_rows(desc, xg, xg_gstride, c, zg, zg_gstride, m, d, Wc, m_pad, s))) return rc;           // :285
+  if ((rc = trsm_right(Lz, ldl, m_pad, Wc, m_pad, c_pad, slices, oz_ws, oz_ws_bytes, s))) return rc;       // :301
+  if (method != 2 && (rc = row_dot_sq(Wc, m_pad, c, m_pad, nullptr, nullptr, q, s))) return rc;           // :305
   sparse_rows_kernel<T><<<(unsigned)nb, 256, 0, s>>>(c, c_pad, kdiag, q, kn, ybar, method, rs, ybs, partial);
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();
@@ -244,7 +206,9 @@ static int sparse_accumulate(const gpk_kernel_desc* desc, const T* xg, int64_t x
   transpose_scaled_kernel<T><<<grid, block, 0, s>>>(Wc, m_pad, c_pad, m_pad, rs, WcT, c_pad);
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();
-  if ((rc = SparseAbi<T>::syrk(m_pad, c_pad, WcT, c_pad, A, lda, slices, oz_ws, oz_ws_bytes, stream))) return rc;                           // :322
+  if ((rc = gemm_nt(m_pad, m_pad, c_pad, T(1), WcT, c_pad, 0, WcT, c_pad, 0, T(1), A, lda, 0, 1, 1, slices, oz_ws,
+                    oz_ws_bytes, s)))  // :322
+    return rc;
   row_dot_acc_kernel<T><<<(unsigned)((m_pad + 7) / 8), 256, 0, s>>>(WcT, c_pad, m_pad, c_pad, ybs, prod);       // :327
   GPK_COUNT_LAUNCH();
   GPK_CHECK_LAUNCH();

@@ -138,6 +138,15 @@ __global__ void dmma_probe_kernel(double* out, int iters, double a, double b) {
   out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
 
+int row_dot_sq(const double* V, int64_t ldv, int64_t rows, int64_t n_cols, const double* b, double* dot, double* sq,
+               cudaStream_t stream) {
+  return gpk_row_dot_sq_f64(V, ldv, 0, rows, n_cols, b, 0, dot, sq, 0, 1, stream);
+}
+int row_dot_sq(const float* V, int64_t ldv, int64_t rows, int64_t n_cols, const float* b, float* dot, float* sq,
+               cudaStream_t stream) {
+  return gpk_row_dot_sq_f32(V, ldv, 0, rows, n_cols, b, 0, dot, sq, 0, 1, stream);
+}
+
 }  // namespace gpk
 
 #define GPK_DEFINE_UTILS(SUF, T)                                                                                       \

@@ -3,11 +3,27 @@
 // the 128 threads of the warpgroup, N / 2 32-bit registers each: register i of thread t is element
 //     row = 16 (t / 32) + (t % 32) / 4 + 8 ((i / 2) % 2),   col = 8 (i / 4) + 2 (t % 4) + (i % 2)
 // so the fragment of columns [32 j, 32 j + 32) is registers [16 j, 16 j + 16): an m64n(32 k) accumulator is k m64n32
-// accumulators side by side.
+// accumulators side by side.  Also the tensor-map encoder both GEMMs build their TMA descriptors with.
 #pragma once
+#include <cuda.h>
+#include <cuda_runtime.h>
 #include <stdint.h>
 
 namespace gpk {
+
+// cuTensorMapEncodeTiled, looked up once through the runtime (the library does not link the driver API); nullptr if absent
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+inline EncodeTiledFn encode_tiled_fn() {
+  static const EncodeTiledFn fn = [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess) return (EncodeTiledFn) nullptr;
+    return (EncodeTiledFn)p;
+  }();
+  return fn;
+}
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }

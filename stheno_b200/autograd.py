@@ -344,6 +344,137 @@ def sparse_elbo(spec, coefs_z, zg_z, ns_z, nv_z, coefs_c, xg_c, zg_c, coefs_x, x
                              params_x)
 
 
+# ---- the sparse ELBO over several processes (PseudoObs with tuples of FDDs) ---------------------------------------------------
+#
+# The same math on the assembled K_z = [k(u_q, u_q')], K_zx = [k(u_q, f_p)], diag K_x = [diag k(f_p)]: only forming the rows
+# and contracting the gradients go block by block.  The forward factors K_z with the lower blocks only, so a block below the
+# diagonal receives dE/dK_z[q, q'] + dE/dK_z[q', q]^T = 2 GK[q, q'] (GK = dE/dK_z is symmetric).
+class MultiSparseElboSpec:
+    """What one multi-output sparse ELBO needs beyond its tensor inputs: the method, ``z_sizes`` (``m_q``) and ``x_sizes``
+    (``n_p``); the nonzero blocks as flat kernels: ``kz`` ``[(q, q', flat)]`` with ``q' <= q``, ``cross`` ``[(p, q, flat)]``
+    (``k(f_p, u_q)``) and ``kx`` ``[(p, flat)]`` (``k(f_p)``, empty for DTC); the chunk; and ``fwd()``, which runs the
+    launches of the no-grad path and returns ``(ch_z, ch_A, s, elbo)``."""
+
+    def __init__(self, method, z_sizes, x_sizes, kz, cross, kx, chunk, fwd):
+        self.method, self.z_sizes, self.x_sizes, self.chunk, self.fwd = method, list(z_sizes), list(x_sizes), chunk, fwd
+        self.kz, self.cross, self.kx = kz, cross, kx
+        self.z_off = [sum(self.z_sizes[:q]) for q in range(len(self.z_sizes))]
+        self.x_off = [sum(self.x_sizes[:p]) for p in range(len(self.x_sizes))]
+
+
+class _MultiSparseElbo(torch.autograd.Function):
+    """Inputs after ``spec``: per ``kz`` block ``(coefs, zg_q, zg_q' or None on the diagonal, params)``, the inducing noise
+    ``nz [m]`` or None, per ``cross`` block ``(coefs, xg_p, zg_q, params)``, per ``kx`` block ``(coefs, xg_p, params)``, then
+    ``kn [n]`` and ``ybar [n]``."""
+
+    @staticmethod
+    def forward(ctx, spec, *ts):
+        ch_z, ch_A, s, elbo = spec.fwd()
+        ctx.spec, ctx.ch_z, ctx.ch_A, ctx.s = spec, ch_z, ch_A, s
+        ctx.ts = [None if t is None else t.detach() for t in ts]
+        return elbo
+
+    @staticmethod
+    def backward(ctx, g):
+        spec, ch_z, ts = ctx.spec, ctx.ch_z, ctx.ts
+        nig = ctx.needs_input_grad[1:]
+        dt, dev, m_pad = ch_z.dtype, ch_z.device, ch_z.n_pad
+        nkz, ncr = len(spec.kz), len(spec.cross)
+        i_nz, i_cr = 4 * nkz, 4 * nkz + 1
+        i_kx = i_cr + 4 * ncr
+        i_kn = i_kx + 3 * len(spec.kx)
+        grads = [None] * len(ts)
+        want_K = any(nig[:i_cr])
+        want_cross = any(nig[i_cr:i_kx])
+
+        def term_buf(i):
+            return torch.zeros(1, _lib.GPK_MAX_TERMS, dtype=dt, device=dev) if nig[i] else None
+
+        # kdiag = diag K_x over all processes (VFE / FITC): what the forward's rows read
+        kdiag = None
+        if spec.method != "dtc":
+            kdiag = torch.zeros(sum(spec.x_sizes), dtype=dt, device=dev)
+            for b, (p, flat) in enumerate(spec.kx):
+                a = spec.x_off[p]
+                kdiag[a : a + spec.x_sizes[p]] = ops.kernel_diag(flat, ts[i_kx + 3 * b + 1])[0]
+
+        procs = [(n_p, []) for n_p in spec.x_sizes]
+        outs = []
+        for b, (p, q, flat) in enumerate(spec.cross):
+            k = i_cr + 4 * b
+            xg, zg = ts[k + 1], ts[k + 2]
+            blk = ops.CrossBlock(flat, xg, zg, spec.z_off[q], term_sum=term_buf(k),
+                                 grad_xg=torch.zeros_like(xg) if nig[k + 1] else None,
+                                 grad_zg=torch.zeros_like(zg) if nig[k + 2] else None,
+                                 param_sum=_param_buf(nig[k + 3], 1, xg))
+            procs[p][1].append(blk)
+            outs.append((k, flat, blk))
+        g_kn, g_kd, g_y, H = ops.sparse_elbo_bwd_multi(procs, ch_z, ctx.ch_A, ctx.s, kdiag, ts[i_kn], ts[i_kn + 1],
+                                                       spec.method, spec.chunk, want_H=want_K, want_cross=want_cross)
+        grads[i_kn], grads[i_kn + 1] = g_kn, g_y
+        for k, flat, blk in outs:
+            grads[k] = None if blk.term_sum is None else blk.term_sum[0, : len(flat.terms)]
+            grads[k + 1], grads[k + 2], grads[k + 3] = blk.grad_xg, blk.grad_zg, _param_grad(flat, blk.param_sum)
+
+        if want_K:
+            # dE/dK_z = -1/2 L^-T H L^-1: two transposed solves with a transpose between them
+            ch_z.solve_many_rows_t_(H)
+            GK = ops.transpose(H, m_pad, m_pad)
+            del H
+            ch_z.solve_many_rows_t_(GK)
+            GK.mul_(-0.5)
+            ops.symmetrize_(GK, m_pad)
+            for b, (q, q2, flat) in enumerate(spec.kz):
+                k = 4 * b
+                if not any(nig[k : k + 4]):
+                    continue
+                o, o2, mq, mq2 = spec.z_off[q], spec.z_off[q2], spec.z_sizes[q], spec.z_sizes[q2]
+                zg, zg2 = ts[k + 1], ts[k + 2]
+                ps = _param_buf(nig[k + 3], 1, zg)
+                if q == q2:
+                    term_sum, g_z, _ = _bwd_kernel(flat, zg, GK[:, o : o + mq, o : o + mq], mq, ps)
+                    grads[k + 1] = g_z if nig[k + 1] else None
+                    scale = 1.0
+                else:
+                    term_sum = torch.zeros(1, _lib.GPK_MAX_TERMS, dtype=dt, device=dev)
+                    g_z = torch.zeros_like(zg) if nig[k + 1] else None
+                    g_z2 = torch.zeros_like(zg2) if nig[k + 2] else None
+                    ops.kernel_cross_bwd(flat, zg, zg2, W=GK[:, o : o + mq, o2 : o2 + mq2], term_sum=term_sum, grad_xsg=g_z,
+                                         grad_xg=g_z2, param_sum=ps)
+                    grads[k + 1], grads[k + 2] = (None if t is None else 2.0 * t for t in (g_z, g_z2))
+                    scale = 2.0
+                grads[k] = scale * term_sum[0, : len(flat.terms)] if nig[k] else None
+                pg = _param_grad(flat, ps)
+                grads[k + 3] = None if pg is None else scale * pg
+            if nig[i_nz]:
+                grads[i_nz] = GK.diagonal(dim1=1, dim2=2)[0, : ch_z.n].clone()
+            del GK
+
+        for b, (p, flat) in enumerate(spec.kx):
+            k = i_kx + 3 * b
+            if not any(nig[k : k + 3]):
+                continue
+            xg = ts[k + 1]
+            ts_x = term_buf(k)
+            g_x = torch.zeros_like(xg) if nig[k + 1] else None
+            ps_x = _param_buf(nig[k + 2], 1, xg)
+            a = spec.x_off[p]
+            ops.kernel_cross_bwd(flat, xg, xg, gdiag=g_kd[a : a + spec.x_sizes[p]].unsqueeze(0), term_sum=ts_x, grad_xsg=g_x,
+                                 param_sum=ps_x)
+            grads[k] = None if ts_x is None else ts_x[0, : len(flat.terms)]
+            grads[k + 1], grads[k + 2] = g_x, _param_grad(flat, ps_x)
+        return (None,) + tuple(None if (gr is None or not w) else g * gr for gr, w in zip(grads, nig))
+
+
+def multi_sparse_elbo(spec, kz, nz, cross, kx, kn, ybar):
+    """The ELBO ``spec.fwd()`` computes for a problem over several processes, differentiable w.r.t. every block's coefficients,
+    pre-stretched inputs and shape parameters (``kz``, ``cross``, ``kx``: one tuple of tensors per block of ``spec``, in
+    :class:`_MultiSparseElbo`'s order), the inducing noise ``nz [m]`` (None: none), the observation noise ``kn [n]`` and
+    ``ybar [n]``."""
+    flat_ts = [t for blk in kz for t in blk] + [nz] + [t for blk in cross for t in blk] + [t for blk in kx for t in blk]
+    return _MultiSparseElbo.apply(spec, *flat_ts, kn, ybar)
+
+
 # ---- exact posterior predictions --------------------------------------------------------------------------------------
 #
 # K = k(x, x) + noise + eps I = L L^T,  alpha = K^-1 ybar,  K* = k(x*, x),  V = K* L^-T,  W = V L^-1 = K* K^-1.

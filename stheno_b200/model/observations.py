@@ -131,6 +131,8 @@ class AbstractPseudoObservations(AbstractObservations):
     def elbo(self, measure):
         if id(measure) not in self._elbo and self._wants_grad(measure):
             e = self._elbo_streamed_grad(measure)
+            if e is None:
+                e = self._elbo_multi_grad(measure)
             if e is not None:
                 self._elbo[id(measure)] = e
         e = self._get(self._elbo, measure)
@@ -237,7 +239,7 @@ class AbstractPseudoObservations(AbstractObservations):
         p_z, z, noise_z = self.u.p, self.u.x, self.u.noise
         if not isinstance(K_n, M.Diagonal) or not isinstance(noise_z, (M.Zero, M.Diagonal)):
             return None
-        if not isinstance(x, Input) or not x.t.is_cuda:
+        if not isinstance(x, Input) or not isinstance(z, Input) or not x.t.is_cuda:
             return None
         K_z = M.add(pairwise(measure.kernels[p_z], z), noise_z)
         if not isinstance(K_z, M.KernelDense) or K_z.xg.shape[1] != 1:
@@ -268,6 +270,72 @@ class AbstractPseudoObservations(AbstractObservations):
         return sparse_elbo(spec, coefs_z, K_z.xg, ns_z, K_z.noise_vec, coef_tensor(flat_c, xg_c), xg_c, zg_c, coefs_x, xg_x,
                            kn, ybar, param_tensor(K_z.flat, K_z.xg), param_tensor(flat_c, xg_c), params_x)
 
+    def _elbo_multi_grad(self, measure):
+        """The ELBO with the analytic backward of ``autograd.multi_sparse_elbo`` when the inducing points and / or the
+        observations span several processes (``self.u.x`` or ``self.fdd.x`` a tuple of FDDs), or None when the problem is not
+        covered: every block ``k(u_q, u_q')``, ``k(u_q, f_p)`` (also symmetric) and, for VFE / FITC, ``k(f_p)`` has to flatten to
+        one descriptor or be zero, no input may have a batch dimension, the noise has to be Diagonal and the inducing noise
+        Zero or Diagonal, and the data have to be on a CUDA device."""
+        from ..autograd import MultiSparseElboSpec, coef_tensor, multi_sparse_elbo, param_tensor
+
+        if not isinstance(self.u.x, tuple) and not isinstance(self.fdd.x, tuple):
+            return None
+        K_n, noise_z = self.fdd.noise, self.u.noise
+        if not isinstance(K_n, M.Diagonal) or not isinstance(noise_z, (M.Zero, M.Diagonal)):
+            return None
+        us, fs = _parts(self.u), _parts(self.fdd)
+        if us is None or fs is None:
+            return None
+        if any(v.batch_shape or not v.t.is_cuda for _, v in us + fs):
+            return None
+        kz, cross, kx = [], [], []
+        spec_kz, spec_cross, spec_kx = [], [], []
+        for q, (pq, zq) in enumerate(us):
+            for q2, (pq2, zq2) in enumerate(us):
+                flat, scales = measure.kernels[pq, pq2]._flat()
+                if flat is None:
+                    return None
+                if q2 <= q and flat.terms:
+                    zg = zq.scaled(scales)
+                    zg2 = None if q2 == q else zq2.scaled(scales)
+                    spec_kz.append((q, q2, flat))
+                    kz.append((coef_tensor(flat, zg), zg, zg2, param_tensor(flat, zg)))
+        for p, (pp, xp) in enumerate(fs):
+            for q, (pq, zq) in enumerate(us):
+                k = measure.kernels[pq, pp]
+                flat, scales = k._flat()
+                if flat is None or not k.symmetric:
+                    return None
+                if flat.terms:
+                    xg = xp.scaled(scales)
+                    spec_cross.append((p, q, flat))
+                    cross.append((coef_tensor(flat, xg), xg, zq.scaled(scales), param_tensor(flat, xg)))
+            if self.method in ("vfe", "fitc"):
+                flat, scales = measure.kernels[pp]._flat()
+                if flat is None:
+                    return None
+                if flat.terms:
+                    xg = xp.scaled(scales)
+                    spec_kx.append((p, flat))
+                    kx.append((coef_tensor(flat, xg), xg, param_tensor(flat, xg)))
+        p_x, x, p_z, z = self.fdd.p, self.fdd.x, self.u.p, self.u.x
+        ybar = (uprank(self.y) - measure.means[p_x].dev(x)).reshape(-1)
+        kn = K_n.diag.reshape(-1)
+        nz = noise_z.diag.reshape(-1) if isinstance(noise_z, M.Diagonal) else None
+
+        def fwd():
+            # the launches of the no-grad route (_compute): the BlockDense factor of K_z, the materialised accumulation
+            K_z = M._densify(M.add(pairwise(measure.kernels[p_z], z), noise_z))
+            if isinstance(K_z, M.KernelDense):
+                K_z.full_precision = True  # one inducing process: never the 7-slice factorisation, as on the single route
+            ch_z = K_z.chol()
+            _, ch_A, sol, elbo, _ = self._elbo_from_factor(measure, ch_z, kn.reshape(1, -1), ybar.reshape(1, -1, 1))
+            return ch_z, ch_A, sol[0, 0], elbo[0]
+
+        spec = MultiSparseElboSpec(self.method, [v.n for _, v in us], [v.n for _, v in fs], spec_kz, spec_cross, spec_kx,
+                                   B.sparse_chunk, fwd)
+        return multi_sparse_elbo(spec, kz, nz, cross, kx, kn, ybar)
+
 
     # -- differentiable route (generic_grad.py): used only when something that feeds the ELBO requires grad -----------------
     def _wants_grad(self, measure):
@@ -278,10 +346,16 @@ class AbstractPseudoObservations(AbstractObservations):
             return False
         p_x, p_z = self.fdd.p, self.u.p
         ks = [measure.kernels[p_z], measure.kernels[p_z, p_x], measure.kernels[p_x]]
+        inputs = [self.fdd.x, self.u.x]
+        if isinstance(self.fdd.x, tuple) or isinstance(self.u.x, tuple):
+            # several processes: the joint kernels do not flatten, so look at the blocks (a mismatched part adds nothing)
+            us, fs = _parts(self.u) or [], _parts(self.fdd) or []
+            ks += [measure.kernels[a, b] for a, _ in us for b, _ in us + fs] + [measure.kernels[b] for b, _ in fs]
+            inputs += [v for _, v in us + fs]
         if any(kernel_needs_grad(k) for k in ks):
             return True
         ts = [self.y]
-        for v in (self.fdd.x, self.u.x):
+        for v in inputs:
             if isinstance(v, Input):
                 ts.append(v.t)
         for nz in (self.fdd.noise, self.u.noise):
@@ -383,6 +457,15 @@ class AbstractPseudoObservations(AbstractObservations):
         det_kn = torch.log(2 * B.pi * kn3).sum(-1)
         yky = (yb3[..., 0] ** 2 / kn3).sum(-1)
         return A, prod, det_kn, yky, trace_part
+
+def _parts(fdd):
+    """``[(process, Input), ...]`` of an FDD over one process or over a tuple of single-process FDDs, else None."""
+    from ..kernels import Input
+
+    parts = [(f.p, f.x) for f in fdd.x] if isinstance(fdd.x, tuple) and all(isinstance(f, FDD) for f in fdd.x) else \
+        [(fdd.p, fdd.x)]
+    return parts if all(isinstance(v, Input) for _, v in parts) else None
+
 
 class PseudoObservations(AbstractPseudoObservations):
     """VFE (Titsias, 2009)."""

@@ -769,6 +769,100 @@ def sparse_elbo_bwd(flat, xg, zg, ch_z, ch_A, s, kdiag, kn, ybar, method, chunk,
     return g_kn, g_kd, g_ybar, H
 
 
+class CrossBlock:
+    """One nonzero block ``k(f_p, u_q)`` of a multi-output sparse problem, for :func:`sparse_elbo_bwd_multi`: its flat kernel,
+    the pre-stretched points ``xg [G, 1, n_p, d]`` of ``f_p`` and ``zg [G, 1, m_q, d]`` of ``u_q``, the first column ``col`` of
+    ``u_q`` in ``K_z``, and the optional outputs ``term_sum``, ``grad_xg`` (like ``xg``), ``grad_zg`` (like ``zg``) and
+    ``param_sum`` the rectangular K1-backward accumulates into (None: not formed)."""
+
+    def __init__(self, flat, xg, zg, col, term_sum=None, grad_xg=None, grad_zg=None, param_sum=None):
+        self.flat, self.xg, self.zg, self.col = flat, xg, zg.contiguous(), int(col)
+        self.term_sum, self.grad_xg, self.grad_zg, self.param_sum = term_sum, grad_xg, grad_zg, param_sum
+
+
+def sparse_elbo_bwd_multi(procs, ch_z, ch_A, s, kdiag, kn, ybar, method, chunk, want_H=True, want_cross=True):
+    """:func:`sparse_elbo_bwd` for inducing points and observations that span several processes.  ``procs``: one entry per
+    observed process ``f_p``, in data order, ``(n_p, [CrossBlock, ...])`` (the nonzero blocks ``k(f_p, u_q)``); ``kdiag``
+    (None for DTC), ``kn`` and ``ybar``: ``[n]`` over all processes.
+
+    The data are walked in chunks of at most ``chunk`` points that never straddle two processes.  A chunk's rows
+    ``k(x_c, z)`` are one ``c_pad x m_pad`` buffer: one K1 launch per block writes exactly ``c x m_q`` entries at the block's
+    column offset (no padding flag: a padded launch would write past ``m_q`` into the next block), and the columns of zero
+    blocks and the ragged rows are zeroed.  The stages after it are those of :func:`sparse_elbo_bwd`; with ``want_cross``
+    the rectangular K1-backward then runs once per block on its column slice of the rows ``dE/dk(x_i, z)``.  Returns
+    ``(g_kn [n], g_kd [n] or None, g_ybar [n], H [1, m_pad, m_pad] or None)``.  Device memory: four ``chunk x m_pad``
+    buffers and three ``m_pad x m_pad`` ones."""
+    _require_cuda(kdiag, kn, ybar)
+    meth = SPARSE_METHOD[method]
+    m, m_pad, dt, dev = ch_z.n, ch_z.n_pad, ch_z.dtype, ch_z.device
+    n = sum(n_p for n_p, _ in procs)
+    V = torch.zeros(1, m_pad, m_pad, dtype=dt, device=dev)
+    V.diagonal(dim1=1, dim2=2).fill_(1.0)
+    ch_A.solve_rows_(V)  # V = L_A^-T, A^-1 = V V^T (the identity on the padding)
+    Ainv = gemm_nt(V, V)
+    del V
+    sp = torch.zeros(m_pad, dtype=dt, device=dev)
+    sp[:m] = s
+    g_kn = torch.empty(n, dtype=dt, device=dev)
+    g_ybar = torch.empty(n, dtype=dt, device=dev)
+    g_kd = torch.empty(n, dtype=dt, device=dev) if meth != 2 else None
+    kdiag, kn, ybar = [None if t is None else t.contiguous() for t in (kdiag, kn, ybar)]
+    H = torch.zeros(1, m_pad, m_pad, dtype=dt, device=dev) if want_H else None
+    rows = round_up(min(int(chunk), max([n_p for n_p, _ in procs] + [1])))
+    Wb = torch.zeros(1, rows, m_pad, dtype=dt, device=dev)  # the padding columns stay zero through the solve
+    Ub = torch.empty(1, rows, m_pad, dtype=dt, device=dev)
+    if want_H:
+        WTb = torch.empty(1, m_pad, rows, dtype=dt, device=dev)
+        GTb = torch.empty(1, m_pad, rows, dtype=dt, device=dev)
+    fn = _fn("gpk_sparse_rows_bwd", dt)
+    a0 = 0
+    for n_p, blocks in procs:
+        gaps, pos = [], 0  # column ranges of zero blocks: the solve of the previous chunk left numbers there
+        for j0, j1 in sorted((blk.col, blk.col + blk.zg.shape[2]) for blk in blocks) + [(m, m)]:
+            if j0 > pos:
+                gaps.append((pos, j0))
+            pos = max(pos, j1)
+        for a in range(0, n_p, int(chunk)):
+            b = min(n_p, a + int(chunk))
+            c, cp = b - a, round_up(b - a)
+            ga, gb = a0 + a, a0 + b
+            Wc, Uc = Wb[:, :cp], Ub[:, :cp]
+            Wc[:, c:].zero_()
+            for j0, j1 in gaps:
+                Wc[:, :c, j0:j1].zero_()
+            for blk in blocks:
+                xc = blk.xg[:, :, a:b].contiguous()
+                Wq = Wc[:, :, blk.col :]
+                _km_launch(blk.flat, xc, blk.zg, c, blk.zg.shape[2], blk.zg.shape[3], 0, 0.0, None, 0.0, Wq, Wq.stride(1),
+                           Wq.stride(0), 1)
+            ch_z.solve_rows_(Wc)
+            q = row_dot_sq(Wc, c, m_pad, None)[1] if meth != 2 else None
+            gemm_nt(Wc, Ainv, Uc)
+            rc = fn(c, m_pad, _ptr(Wc), Wc.stride(1), _ptr(Uc), Uc.stride(1), _ptr(sp), _ptr(q),
+                    _ptr(None if kdiag is None else kdiag[ga:gb]), _ptr(kn[ga:gb]), _ptr(ybar[ga:gb]), meth, _ptr(g_kn[ga:gb]),
+                    _ptr(None if g_kd is None else g_kd[ga:gb]), _ptr(g_ybar[ga:gb]), _stream())
+            check(rc, "gpk_sparse_rows_bwd")
+            if want_H:
+                WT, GT = WTb[:, :, :cp], GTb[:, :, :cp]
+                transpose(Wc, cp, m_pad, out=WT)
+                transpose(Uc, cp, m_pad, out=GT)
+                gemm_nt(GT, WT, H, beta=1.0, lower=True)
+            if want_cross and blocks:
+                ch_z.solve_many_rows_t_(Uc)
+                for blk in blocks:
+                    xc = blk.xg[:, :, a:b].contiguous()
+                    mq = blk.zg.shape[2]
+                    gx = torch.zeros_like(xc) if blk.grad_xg is not None else None
+                    kernel_cross_bwd(blk.flat, xc, blk.zg, W=Uc[:, :, blk.col : blk.col + mq], term_sum=blk.term_sum,
+                                     grad_xsg=gx, grad_xg=blk.grad_zg, param_sum=blk.param_sum)
+                    if gx is not None:
+                        blk.grad_xg[:, :, a:b] += gx
+        a0 += n_p
+    if want_H:
+        symmetrize_(H, m_pad)
+    return g_kn, g_kd, g_ybar, H
+
+
 def gemm_profile(enable):
     """Switch the in-situ event timing of the fp64 GEMM kernel on / off (clears the record)."""
     _lib.load().gpk_gemm_profile_enable(1 if enable else 0)

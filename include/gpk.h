@@ -289,6 +289,21 @@ int gpk_sparse_posterior_marginals_f32(const gpk_kernel_desc* desc_host, const f
                                        const float* LS, int64_t ldls, int64_t m_pad, const float* half_y, float* dot,
                                        float* sq_z, float* sq_s, int64_t chunk, float* ws, int64_t ws_elems, void* stream);
 
+/* Backward of gpk_sparse_posterior_marginals in the test inputs, the per-test-point step of one chunk of `c` points (rows;
+ * c_pad = round_up(c)).  In: V, U [c_pad x m_pad] (same ld) the solved rows v_i^T = k(x*_i, z) L_z^-T and
+ * u_i^T = k(x*_i, z) L_S^-T as the forward leaves them, h [m_pad] = half_y (zero padded), a [c] the upstream gradient of
+ * dot (mean) and b [c] that of the variance (k - sq_z) + sq_s; either of a and b may be NULL (zero), not both; h may be
+ * NULL when a is.  In place:
+ *   row i of V <- a_i h - 2 b_i v_i,   row i of U <- 2 b_i u_i;   rows c .. c_pad - 1 of V and U are zeroed.
+ * V and U are read only when b is given (without it they may hold anything: V becomes a_i h, U zero).
+ * The caller finishes dL/dk(x*_i, z) = L_z^-T (row i of V) + L_S^-T (row i of U) with two transposed solves and contracts
+ * it with dk/dx* in the rectangular K1-backward (gpk_kernel_cross_bwd).  One warp per row, fp64 arithmetic in both
+ * precisions. */
+int gpk_sparse_posterior_rows_bwd_f64(int64_t c, int64_t m_pad, double* V, double* U, int64_t ld, const double* h,
+                                      const double* a, const double* b, void* stream);
+int gpk_sparse_posterior_rows_bwd_f32(int64_t c, int64_t m_pad, float* V, float* U, int64_t ld, const float* h, const float* a,
+                                      const float* b, void* stream);
+
 /* Streamed sparse (inducing-point) accumulation -- AbstractPseudoObservations._compute, stheno/model/observations.py:279-336,
  * one chunk of `c` data points per call; K_zx (8.6 GB at n = 262144, m = 4096) is never held.  Per chunk, stream-ordered:
  *   W_c^T = k(x_c, z) L_z^-T  (:285, :301; rows = data points, [c_pad x m_pad], c_pad = round_up(c))

@@ -18,7 +18,7 @@ import torch
 from . import _lib, ops
 
 __all__ = ["kernel_logpdf", "dense_logpdf", "kernel_matrix_grad", "kernel_cross_grad", "kernel_diag_grad", "exact_posterior",
-           "no_gradient"]
+           "sparse_posterior_marginals", "subspace_cov", "no_gradient"]
 
 
 def _bwd_kernel(flat, xg, G, n, param_sum=None):
@@ -473,6 +473,91 @@ def multi_sparse_elbo(spec, kz, nz, cross, kx, kn, ybar):
     ``ybar [n]``."""
     flat_ts = [t for blk in kz for t in blk] + [nz] + [t for blk in cross for t in blk] + [t for blk in kx for t in blk]
     return _MultiSparseElbo.apply(spec, *flat_ts, kn, ybar)
+
+
+# ---- sparse posterior predictions in the test inputs ------------------------------------------------------------------------
+#
+# PseudoObs* posteriors: r_i = k(x*_i, z), v_i = L_z^-1 r_i, u_i = L_S^-1 r_i (L_S: the factor of the stored A + eps I),
+# mean_i = m(x*_i) + <v_i, h>, var_i = k(x*_i, x*_i) - |v_i|^2 + |u_i|^2, C = P - V V^T + U U^T.  With K_z, A and mu constant
+# (nothing that feeds the approximation requires grad) the gradient in x* needs only the factors the forward holds:
+#   dL/dr_i = L_z^-T (a_i h - 2 b_i v_i) + L_S^-T (2 b_i u_i)          (marginals; a, b: upstream of mean, var)
+#   dL/dR   = (2 Hs U) L_S^-1 for the U U^T term of C, Hs = (gC + gC^T) / 2 (the P - V V^T term is exact_posterior's)
+# The derivative of what the forward computes, eps included; the prior terms m(x*), k(x*, x*) and P keep their own graphs.
+class SparsePosteriorSpec:
+    """What the sparse marginals need beyond the test points: the cross kernel ``flat`` and the pre-stretched inducing points
+    ``zg``, the factors ``ch_z`` of ``K_z`` and ``ch_s`` of the stored ``A`` (+ eps I), ``half_y = L_z^-1 (mu - m_z(z))``
+    (``[m_pad]``; None: variances only) and the chunk of test points."""
+
+    def __init__(self, flat, zg, ch_z, ch_s, half_y, chunk=4096):
+        self.flat, self.zg, self.ch_z, self.ch_s, self.half_y, self.chunk = flat, zg, ch_z, ch_s, half_y, chunk
+
+
+class _SparsePosteriorMarginals(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, spec, xsg, prior_m, prior_v):
+        ctx.set_materialize_grads(False)
+        ctx.spec, ctx.xsg = spec, xsg.detach()
+        ctx.shapes = (None if prior_m is None else prior_m.shape, prior_v.shape)
+        dot, sq_z, sq_s = ops.sparse_posterior_marginals(spec.flat, ctx.xsg, spec.zg, spec.ch_z, spec.ch_s, spec.half_y,
+                                                         want_dot=spec.half_y is not None, chunk=spec.chunk)
+        n = xsg.shape[2]
+        var = (prior_v - sq_z.reshape(n, 1)) + sq_s.reshape(n, 1)
+        if prior_m is None:
+            mean = xsg.new_empty(0)
+            ctx.mark_non_differentiable(mean)
+        else:
+            mean = prior_m + dot.reshape(n, 1)
+        return mean, var
+
+    @staticmethod
+    def backward(ctx, g_mean, g_var):
+        spec, xsg = ctx.spec, ctx.xsg
+        _, want_xs, want_pm, want_pv = ctx.needs_input_grad
+        grad_xs = None
+        if want_xs and (g_mean is not None or g_var is not None):
+            grad_xs = ops.sparse_posterior_marginals_bwd(spec.flat, xsg, spec.zg, spec.ch_z, spec.ch_s, spec.half_y, g_mean,
+                                                         g_var, chunk=spec.chunk)
+        shape_m, shape_v = ctx.shapes
+        grad_pm = g_mean.sum_to_size(shape_m) if (want_pm and g_mean is not None) else None
+        grad_pv = g_var.sum_to_size(shape_v) if (want_pv and g_var is not None) else None
+        return None, grad_xs, grad_pm, grad_pv
+
+
+def sparse_posterior_marginals(spec, xsg, prior_m, prior_v):
+    """``(mean, var)`` of a sparse posterior at the pre-stretched test points ``xsg [G, 1, n*, d]``: ``prior_m + dot`` (an empty
+    tensor when ``prior_m`` is None) and ``(prior_v - sq_z) + sq_s``, each ``[n*, 1]``, from ``ops.sparse_posterior_marginals``.
+    Differentiable w.r.t. ``xsg`` (the factors are constants) and, unchanged, w.r.t. the prior terms ``prior_m`` and
+    ``prior_v [n*, 1]``."""
+    return _SparsePosteriorMarginals.apply(spec, xsg, prior_m, prior_v)
+
+
+class _SubspaceCov(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, ch, flat, zg, xsg, fwd):
+        C, U = fwd()
+        ctx.ch, ctx.flat, ctx.zg, ctx.xsg, ctx.U = ch, flat, zg, xsg.detach(), U
+        return C
+
+    @staticmethod
+    def backward(ctx, gC):
+        U, xsg = ctx.U, ctx.xsg
+        m, mp, m_pad = xsg.shape[2], U.shape[1], U.shape[2]
+        g = gC.reshape(1, m, m)
+        D2 = torch.zeros(1, mp, mp, dtype=U.dtype, device=U.device)
+        D2[:, :m, :m] = g + g.transpose(1, 2)  # 2 Hs
+        Y = ops.gemm_nt(D2, ops.transpose(U, mp, m_pad))  # 2 Hs U
+        del D2
+        ctx.ch.solve_many_rows_t_(Y)
+        grad_xs = torch.zeros_like(xsg)
+        ops.kernel_cross_bwd(ctx.flat, xsg, ctx.zg, W=Y, grad_xsg=grad_xs)
+        return None, None, None, grad_xs, None
+
+
+def subspace_cov(ch, flat, zg, xsg, fwd):
+    """``U U^T`` as ``fwd()`` computes it -- ``fwd`` returns ``(C, U)`` with ``U = k(x*, z) L_S^-T`` the padded solved rows
+    ``[1, m_pad*, m_pad]`` and ``ch`` the factor ``L_S`` -- differentiable w.r.t. the pre-stretched test points ``xsg`` of the
+    cross kernel ``flat`` (``zg``: its pre-stretched inducing points; the factor is a constant)."""
+    return _SubspaceCov.apply(ch, flat, zg, xsg, fwd)
 
 
 # ---- exact posterior predictions --------------------------------------------------------------------------------------

@@ -100,9 +100,60 @@ static int sparse_posterior_marginals(const gpk_kernel_desc* desc, const T* xsg,
   return 0;
 }
 
+// Backward of the sparse marginals in the test inputs, per test point of a chunk (one warp per row): with the upstream
+// gradients a_i of dot_i and b_i of the variance (k - sq_z) + sq_s, the rows of dL/dk(x*_i, z) are
+// L_z^-T (a_i h - 2 b_i v_i) + L_S^-T (2 b_i u_i); this writes the two right-hand sides over V and U and zeroes the ragged rows.
+template <typename T>
+__global__ void sparse_post_rows_bwd_kernel(int64_t c, int64_t c_pad, int64_t m_pad, T* __restrict__ V, T* __restrict__ U,
+                                            int64_t ld, const T* __restrict__ h, const T* __restrict__ a,
+                                            const T* __restrict__ b) {
+  const int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (i >= c_pad) return;
+  const int lane = threadIdx.x & 31;
+  T* v = V + i * ld;
+  T* u = U + i * ld;
+  if (i >= c) {
+    for (int64_t j = lane; j < m_pad; j += 32) v[j] = u[j] = T(0);
+    return;
+  }
+  // V and U are read only when b is given: without it the caller need not have formed them
+  const double ai = a ? (double)a[i] : 0.0;
+  const double b2 = b ? 2.0 * (double)b[i] : 0.0;
+  for (int64_t j = lane; j < m_pad; j += 32) {
+    double vj = a ? ai * (double)h[j] : 0.0;
+    double uj = 0.0;
+    if (b) {
+      vj = fma(-b2, (double)v[j], vj);
+      uj = b2 * (double)u[j];
+    }
+    v[j] = (T)vj;
+    u[j] = (T)uj;
+  }
+}
+
+template <typename T>
+static int sparse_posterior_rows_bwd(int64_t c, int64_t m_pad, T* V, T* U, int64_t ld, const T* h, const T* a, const T* b,
+                                     void* stream) {
+  if (!V || !U || c < 1 || m_pad < 128 || m_pad % 128 || ld < m_pad) return GPK_ERR_ARG;
+  if ((!a && !b) || (a && !h)) return GPK_ERR_ARG;
+  const int64_t c_pad = (c + 127) / 128 * 128;
+  sparse_post_rows_bwd_kernel<T><<<(unsigned)(c_pad / 8), 256, 0, (cudaStream_t)stream>>>(c, c_pad, m_pad, V, U, ld, h, a, b);
+  GPK_COUNT_LAUNCH();
+  GPK_CHECK_LAUNCH();
+  return 0;
+}
+
 }  // namespace gpk
 
 extern "C" {
+int gpk_sparse_posterior_rows_bwd_f64(int64_t c, int64_t m_pad, double* V, double* U, int64_t ld, const double* h,
+                                      const double* a, const double* b, void* stream) {
+  return gpk::sparse_posterior_rows_bwd<double>(c, m_pad, V, U, ld, h, a, b, stream);
+}
+int gpk_sparse_posterior_rows_bwd_f32(int64_t c, int64_t m_pad, float* V, float* U, int64_t ld, const float* h, const float* a,
+                                      const float* b, void* stream) {
+  return gpk::sparse_posterior_rows_bwd<float>(c, m_pad, V, U, ld, h, a, b, stream);
+}
 int64_t gpk_sparse_posterior_ws_elems(int64_t chunk, int64_t m_pad) { return 2 * ((chunk + 127) / 128 * 128) * m_pad; }
 int gpk_sparse_posterior_marginals_f64(const gpk_kernel_desc* desc_host, const double* xsg, int64_t xsg_gstride, int64_t ns,
                                        const double* zg, int64_t zg_gstride, int64_t m, int32_t d, const double* Lz,

@@ -1133,12 +1133,35 @@ class SubspaceKernel(Kernel):
 
     def _pairwise_any(self, x, y, same):
         org = _origin_of_input(x)
-        Vx, mx = self._half(self.k_zi, x)
         same_half = same and (self.k_zi is self.k_zj)
-        Vy, my = (Vx, mx) if same_half else self._half(self.k_zj, x if same else y)
-        C = ops.gemm_nt(Vx, Vy, lower=False)
-        bs = _batch_shape_of_input(x)
-        return M.Dense(self._no_grad(C[:, :mx, :my].reshape(bs + (mx, my)), x, y), org)
+
+        def fwd():
+            Vx, mx = self._half(self.k_zi, x)
+            Vy, my = (Vx, mx) if same_half else self._half(self.k_zj, x if same else y)
+            C = ops.gemm_nt(Vx, Vy, lower=False)
+            return C[:, :mx, :my].reshape(_batch_shape_of_input(x) + (mx, my)), Vx
+
+        route = self._xs_route(x) if same_half else None
+        if route is not None:
+            from .autograd import subspace_cov
+
+            return M.Dense(subspace_cov(self.A.chol(), *route, fwd), org)
+        return M.Dense(self._no_grad(fwd()[0], x, y), org)
+
+    def _xs_route(self, x):
+        """``(flat, zg, xsg)`` when the covariance at ``x`` has an analytic gradient in ``x``: only ``x`` requires grad, the
+        cross kernel flattens to one descriptor, and ``x``, ``z`` and ``A`` are single-output and unbatched; else None."""
+        if _grad_tensors(self.A, self.k_zi, self.z) or not _grad_tensors(x):
+            return None
+        if _is_multi(x) or _is_multi(self.z) or not self.k_zi.symmetric:
+            return None
+        xi, zi = as_input(x), as_input(self.z)
+        if xi.batch_shape or zi.batch_shape or self.A.chol().batch != 1:
+            return None
+        flat, scales = self.k_zi._flat()
+        if flat is None or not flat.terms:
+            return None
+        return flat, zi.scaled(scales), xi.scaled(scales)
 
     def _elwise_any(self, x, y, same):
         Vx, mx = self._half(self.k_zi, x)
@@ -1490,7 +1513,8 @@ def _shared_posterior(mean, kernel):
 def _sparse_posterior(mean, kernel, x):
     """The sparse counterpart of :func:`_shared_posterior`: the ``PosteriorMean`` and ``PosteriorKernel + SubspaceKernel`` of
     one ``PseudoObs*`` problem (``AbstractPseudoObservations``) at numeric, single-output, unbatched ``x``, with one cross
-    kernel that flattens to one descriptor and nothing that requires grad -- the marginals :func:`_sparse_marginals` streams."""
+    kernel that flattens to one descriptor and nothing that requires grad except ``x`` itself -- the marginals
+    :func:`_sparse_marginals` streams, differentiable in ``x``."""
     if not (isinstance(mean, PosteriorMean) and isinstance(kernel, SumKernel)):
         return False
     pk, sk, k = kernel.a, kernel.b, mean.k_zi
@@ -1505,29 +1529,31 @@ def _sparse_posterior(mean, kernel, x):
     flat, _ = k._flat()
     if flat is None or not flat.terms:
         return False
-    if _grad_tensors(mean, kernel, x):
+    if _grad_tensors(mean, kernel):
         return False
     return mean.K_z.chol().batch == 1 and sk.A.chol().batch == 1
 
 
 def _sparse_marginals(mean, kernel, x, want_dot):
-    """``(dot, sq_z, sq_s)`` of a posterior :func:`_sparse_posterior` accepts, each ``[..., n, 1]``: the K1 rows at ``x``
-    are formed once per chunk of test points and solved against ``L_z`` and against the factor of ``A`` (``dot`` None unless
-    ``want_dot``)."""
+    """``(mean or None, var)`` of a posterior :func:`_sparse_posterior` accepts, each ``[n, 1]``: the K1 rows at ``x`` are
+    formed once per chunk of test points and solved against ``L_z`` and against the factor of ``A`` (the mean only with
+    ``want_dot``); differentiable in ``x`` (``autograd.sparse_posterior_marginals``)."""
+    from .autograd import SparsePosteriorSpec, sparse_posterior_marginals
+
     xi, zi = as_input(x), as_input(mean.z)
     flat, scales = mean.k_zi._flat()
-    half_y = mean._half_y()[0] if want_dot else None
-    out = ops.sparse_posterior_marginals(flat, xi.scaled(scales), zi.scaled(scales), mean.K_z.chol(), kernel.b.A.chol(),
-                                         half_y, want_dot=want_dot)
-    return tuple(None if t is None else t.reshape(xi.n, 1) for t in out)
+    spec = SparsePosteriorSpec(flat, zi.scaled(scales), mean.K_z.chol(), kernel.b.A.chol(),
+                               mean._half_y()[0] if want_dot else None)
+    prior_m = mean.m_i.dev(x) if want_dot else None
+    mu, var = sparse_posterior_marginals(spec, xi.scaled(scales), prior_m, _elwise_any(kernel.a.k_ij, x, None, True))
+    return (mu if want_dot else None), var
 
 
 def marginal_var(mean, kernel, x):
     """``k.elwise(x)`` of a posterior process with mean ``mean``, ``[..., n, 1]``: the streamed sparse marginals where
     :func:`_sparse_posterior` holds, else the kernel's own element-wise evaluation."""
     if _sparse_posterior(mean, kernel, x):
-        _, sq_z, sq_s = _sparse_marginals(mean, kernel, x, want_dot=False)
-        return (_elwise_any(kernel.a.k_ij, x, None, True) - sq_z) + sq_s
+        return _sparse_marginals(mean, kernel, x, want_dot=False)[1]
     return _elwise_any(kernel, x, None, True)
 
 
@@ -1585,6 +1611,5 @@ def mean_var_diag(mean, kernel, x):
             dot, sq, _ = _exact_posterior(mean.K_z, route[0], mean._ybar(), fwd, half_y=mean._half_y())
         return prior_m + dot.reshape(shp).unsqueeze(-1), prior_v - sq.reshape(shp).unsqueeze(-1)
     if _sparse_posterior(mean, kernel, x):
-        dot, sq_z, sq_s = _sparse_marginals(mean, kernel, x, want_dot=True)
-        return mean.m_i.dev(x) + dot, (_elwise_any(kernel.a.k_ij, x, None, True) - sq_z) + sq_s
+        return _sparse_marginals(mean, kernel, x, want_dot=True)
     return mean.dev(x), _elwise_any(kernel, x, None, True)

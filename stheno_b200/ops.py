@@ -648,6 +648,56 @@ def sparse_posterior_marginals(flat, xsg, zg, ch_z, ch_s, half_y, want_dot=True,
     return dot, sq_z, sq_s
 
 
+def sparse_posterior_marginals_bwd(flat, xsg, zg, ch_z, ch_s, half_y, a, b, chunk=4096):
+    """Gradient w.r.t. ``xsg`` of :func:`sparse_posterior_marginals` for the upstream gradients ``a [n*]`` of the mean (``dot``)
+    and ``b [n*]`` of the variance ``(k - sq_z) + sq_s`` (either may be None).  The factors are constants: with
+    ``r_i = k(x*_i, z)``, ``dL/dr_i = L_z^-T (a_i h - 2 b_i v_i) + L_S^-T (2 b_i u_i)``.  Per chunk of test points, as the forward
+    walks them: K1 rows into ``V``, copied to ``U``, the right solves against ``L_z`` and ``L_S``, ``gpk_sparse_posterior_rows_bwd``,
+    the transposed solves, ``V += U`` and the rectangular K1-backward.  Returns ``grad_xsg`` (like ``xsg``).  Device memory: two
+    ``chunk x m_pad`` buffers and the copies the transposed solves make, whatever ``n*`` is."""
+    _check_groups(zg, flat)
+    _require_cuda(xsg, zg, half_y, a, b)
+    if ch_z.batch != 1 or ch_s.batch != 1 or xsg.shape[1] != 1 or zg.shape[1] != 1:
+        raise ValueError("sparse_posterior_marginals_bwd handles a single problem")
+    if ch_s.n_pad != ch_z.n_pad or zg.shape[2] != ch_z.n:
+        raise ValueError("sparse_posterior_marginals_bwd: the factors and the inducing points do not match")
+    if a is None and b is None:
+        raise ValueError("sparse_posterior_marginals_bwd needs an upstream gradient")
+    xsg, zg = xsg.contiguous(), zg.contiguous()
+    ns, d = xsg.shape[2], xsg.shape[3]
+    dt, dev, m, m_pad = ch_z.dtype, ch_z.device, ch_z.n, ch_z.n_pad
+    grad = torch.zeros_like(xsg)
+    if ns == 0:
+        return grad
+    a, b = [None if t is None else t.reshape(-1).contiguous() for t in (a, b)]
+    hy = half_y.contiguous() if a is not None else None
+    chunk = min(round_up(chunk), round_up(ns))
+    Vb = torch.empty(1, chunk, m_pad, dtype=dt, device=dev)
+    Ub = torch.empty(1, chunk, m_pad, dtype=dt, device=dev)
+    fn = _fn("gpk_sparse_posterior_rows_bwd", dt)
+    for c0 in range(0, ns, chunk):
+        c1 = min(ns, c0 + chunk)
+        c, cp = c1 - c0, round_up(c1 - c0)
+        xs_c = xsg[:, :, c0:c1].contiguous()
+        V, U = Vb[:, :cp], Ub[:, :cp]
+        if b is not None:  # without a variance upstream the rows kernel reads neither buffer
+            _km_launch(flat, xs_c, zg, c, m, d, KM_PAD_ZERO, 0.0, None, 0.0, V, V.stride(1), V.stride(0), 1)
+            U.copy_(V)
+            ch_z.solve_rows_(V)
+            ch_s.solve_rows_(U)
+        rc = fn(c, m_pad, _ptr(V), _ptr(U), V.stride(1), _ptr(hy), _ptr(None if a is None else a[c0:c1]),
+                _ptr(None if b is None else b[c0:c1]), _stream())
+        check(rc, "gpk_sparse_posterior_rows_bwd")
+        ch_z.solve_many_rows_t_(V)
+        if b is not None:  # else U is zero
+            ch_s.solve_many_rows_t_(U)
+            V += U
+        gx = torch.zeros_like(xs_c)
+        kernel_cross_bwd(flat, xs_c, zg, W=V, grad_xsg=gx)
+        grad[:, :, c0:c1] = gx
+    return grad
+
+
 SPARSE_METHOD = {"vfe": 0, "fitc": 1, "dtc": 2}
 
 

@@ -272,7 +272,8 @@ def no_gradient(route, value, inputs):
 class SparseElboSpec:
     """What one sparse ELBO needs beyond its tensor inputs: the method, the flat kernels of ``K_z`` (``flat_z``), of the cross
     kernel (``flat_c``) and of ``k_x`` (``flat_x``, None for DTC), the chunk, and ``fwd()``, which runs the launches of the
-    no-grad streamed path and returns ``(ch_z, ch_A, s, kdiag, elbo)``."""
+    no-grad path and returns ``(ch_z, ch_A, s, kdiag, elbo)`` (``kdiag`` None where that path does not stream: the backward
+    then forms ``diag K_x`` itself)."""
 
     def __init__(self, method, flat_z, flat_c, flat_x, chunk, fwd):
         self.method, self.flat_z, self.flat_c, self.flat_x, self.chunk, self.fwd = method, flat_z, flat_c, flat_x, chunk, fwd
@@ -301,8 +302,11 @@ class _SparseElbo(torch.autograd.Function):
         g_xc = torch.zeros_like(ctx.xg_c) if want_xg_c else None
         g_zc = torch.zeros_like(ctx.zg_c) if want_zg_c else None
         ps_c = _param_buf(want_params_c, 1, ctx.xg_c)
+        kdiag = ctx.kdiag
+        if kdiag is None and spec.method != "dtc":  # the materialised forward (input-mapped kernels) did not keep diag K_x
+            kdiag = ops.kernel_diag(spec.flat_x, ctx.xg_x)[0]
         g_kn, g_kd, g_y, H = ops.sparse_elbo_bwd(
-            spec.flat_c, ctx.xg_c, ctx.zg_c, ch_z, ctx.ch_A, ctx.s, ctx.kdiag, ctx.kn, ctx.ybar, spec.method, spec.chunk,
+            spec.flat_c, ctx.xg_c, ctx.zg_c, ch_z, ctx.ch_A, ctx.s, kdiag, ctx.kn, ctx.ybar, spec.method, spec.chunk,
             want_H=want_K, want_cross=want_coefs_c or want_xg_c or want_zg_c or want_params_c, term_sum=ts_c, grad_xg=g_xc,
             grad_zg=g_zc, param_sum=ps_c)
         grads = dict(kn=g_kn, ybar=g_y, coefs_c=None if ts_c is None else ts_c[0, : len(spec.flat_c.terms)], xg_c=g_xc,

@@ -766,6 +766,68 @@ def _map_kernel(k, kind, params):
     return MappedKernel(k, m1, m2)
 
 
+def flat_under_maps(k, x, y=None):
+    """``k(x, y)`` as one flat kernel at mapped points, for the analytic gradient routes: ``(flat, scales, xm, ym)`` with
+    ``flat, scales`` the :meth:`Kernel._flat` of the kernel inside a chain of :class:`MappedKernel` s (``shift``, ``stretch``,
+    ``select``, ``periodic``, ``transform``, nested in any order; no chain: ``k`` itself) and ``xm``, ``ym`` the
+    :class:`Input` s the chain makes of ``x`` and ``y``, with their torch graph to the raw points and to the maps' parameters.
+    ``y=None``: the square ``k(x, x)``, whose two maps must be equal at every link (then ``ym is xm``); else each argument
+    takes its own maps.  None when the kernel inside does not flatten to one descriptor with terms (sums or products of
+    differently mapped kernels, derivatives, ...)."""
+    maps = []
+    while isinstance(k, MappedKernel):
+        if y is None and not _same_map(k.m1, k.m2):
+            return None
+        maps.append((k.m1, k.m2))
+        k = k.k
+    flat, scales = k._flat()
+    if flat is None or not flat.terms:
+        return None
+    xm = as_input(x)
+    ym = xm if y is None else as_input(y)
+    for m1, m2 in maps:  # outermost first: MappedKernel(k, m1, m2)(x, y) = k(m1(x), m2(y))
+        if y is None:
+            xm = ym = xm if m1 is None else m1(xm)
+        else:
+            xm, ym = (xm if m1 is None else m1(xm)), (ym if m2 is None else m2(ym))
+    return flat, scales, xm, ym
+
+
+def _children(k):
+    return [c for c in (getattr(k, "k", None), getattr(k, "a", None), getattr(k, "b", None)) if isinstance(c, Kernel)]
+
+
+def _maps(k):
+    """The input maps anywhere inside the kernel expression ``k``."""
+    out = [m for m in ((k.m1, k.m2) if isinstance(k, MappedKernel) else ()) if m is not None]
+    for c in _children(k):
+        out += _maps(c)
+    return out
+
+
+def map_output_grads(k, x, y):
+    """The points that ``k``'s ``transform`` maps produce from the arguments of ``k(x, y)`` and that require grad.  A transform's
+    parameters (a network's weights) hide in its closure, so only its output shows that the kernel depends on them: the maps
+    are evaluated here (O(n d)).  Empty when grad mode is off or ``k`` has no transform; the other maps' parameters are
+    tensors :func:`_grad_tensors` finds."""
+    if not torch.is_grad_enabled() or not any(m.kind == "transform" for m in _maps(k)):
+        return []
+    out = []
+
+    def walk(k, x, y):
+        if isinstance(k, MappedKernel):
+            x, y = (x if k.m1 is None else k.m1(x)), (y if k.m2 is None else k.m2(y))
+            out.extend(t for t in (x.t, y.t) if t.requires_grad)
+        elif isinstance(k, ReversedKernel):
+            x, y = y, x
+        for c in _children(k):
+            if _maps(c):
+                walk(c, x, y)
+
+    walk(k, as_input(x), as_input(y))
+    return out
+
+
 class DerivativeKernel(Kernel):
     """``d^a/dx_{d1} d^b/dy_{d2} k(x, y)`` (``a, b`` in {0, 1}; mlkernels ``DerivativeKernel`` behind ``GP.diff``,
     ``stheno/model/measure.py:343-360``).  Evaluated by forward-mode differentiation (``torch.func.jvp``, nested for the mixed
@@ -991,17 +1053,16 @@ def _grad_tensors(*objs):
 def _exact_route(K_z, k_zi, z, x, *others):
     """How a posterior prediction at ``x`` is evaluated: None when no gradient is requested (the raw-pointer path), else
     ``(args, tensors)`` -- ``args`` the inputs of :func:`autograd.exact_posterior` when the posterior is covered (exact
-    observations with a symbolic ``K_z``, a symmetric cross kernel that flattens to one descriptor, single-output inputs of
-    the factor's batch), None when it is not."""
-    ts = _grad_tensors(K_z, k_zi, z, x, *others)
+    observations with a symbolic ``K_z``, a cross kernel that is one flat descriptor under input maps
+    (:func:`flat_under_maps`), single-output inputs of the factor's batch), None when it is not."""
+    multi = _is_multi(x) or _is_multi(z)
+    ts = _grad_tensors(K_z, k_zi, z, x, *others) + ([] if multi else map_output_grads(k_zi, z, x))
     if not ts:
         return None
-    if not isinstance(K_z, M.KernelDense) or _is_multi(x) or _is_multi(z) or not k_zi.symmetric:
+    res = None if multi or not isinstance(K_z, M.KernelDense) else flat_under_maps(k_zi, z, x)
+    if res is None:
         return None, ts
-    flat, scales = k_zi._flat()
-    if flat is None or not flat.terms:
-        return None, ts
-    xi, zi = as_input(x), as_input(z)
+    flat, scales, zi, xi = res
     xsg, zg = xi.scaled(scales), zi.scaled(scales)
     if xsg.shape[1] != K_z.xg.shape[1] or zg.shape[1] != K_z.xg.shape[1] or zg.shape[2] != K_z.n:
         return None, ts
@@ -1494,8 +1555,8 @@ def _route_name(post):
     if isinstance(K_z, M.BlockDense) or isinstance(post.z, (tuple, FDD)):
         return "multi-output posterior"
     if isinstance(K_z, M.KernelDense):
-        return "posterior whose cross kernel is not one flat kernel expression (input maps, derivatives, periodic, " \
-               "function-scaled, reversed) or whose inputs are multi-output or of another batch"
+        return "posterior whose cross kernel is not one flat kernel expression under input maps (derivatives, " \
+               "function-scaled, reversed, sums of differently mapped kernels) or whose inputs are multi-output or of another batch"
     return "sparse (pseudo-observation) or non-kernel posterior"
 
 

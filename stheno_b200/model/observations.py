@@ -6,7 +6,7 @@ import torch
 from .. import B
 from .. import matrix as M
 from .. import ops
-from ..kernels import (PosteriorKernel, PosteriorMean, SubspaceKernel, _cross_rows, _elwise_any, num_elements,
+from ..kernels import (PosteriorKernel, PosteriorMean, SubspaceKernel, _cross_rows, _elwise_any, _maps, num_elements,
                        pairwise)
 from .._util import batch_flatten, from_dev, to_dev, uprank
 from .fdd import FDD, _input_meta
@@ -174,7 +174,7 @@ class AbstractPseudoObservations(AbstractObservations):
         p_x, x, noise_x = self.fdd.p, self.fdd.x, self.fdd.noise
         p_z, z, noise_z = self.u.p, self.u.x, self.u.noise
         if self._wants_grad(measure):
-            return self._compute_grad(measure)
+            return self._compute_uncovered(measure) if self._mapped(measure) else self._compute_grad(measure)
         K_z = M.add(pairwise(measure.kernels[p_z], z), noise_z)  # :286
         self._K_z.setdefault(id(measure), K_z)
         K_n = noise_x  # :290
@@ -230,10 +230,12 @@ class AbstractPseudoObservations(AbstractObservations):
     # -- analytic streamed gradient (autograd.sparse_elbo): the ELBO under grad of one problem on the GPU ---------------------
     def _elbo_streamed_grad(self, measure):
         """The ELBO with the analytic backward of ``autograd.sparse_elbo``, or None when the problem is not covered: it needs
-        the streamed route (:meth:`_stream_plan`), ``k_z`` and ``k_x`` that each flatten to one descriptor, Diagonal noise,
-        Zero or Diagonal inducing noise, and data on a CUDA device."""
+        one problem of numeric inputs, ``k_z``, a symmetric ``k_zx`` and ``k_x`` that are each one flat descriptor under input
+        maps (:func:`kernels.flat_under_maps`), Diagonal noise, Zero or Diagonal inducing noise, and data on a CUDA device.
+        The backward streams the rows of ``k_zx`` at the mapped points; the forward runs the no-grad launches (for mapped
+        kernels the materialised accumulation)."""
         from ..autograd import SparseElboSpec, coef_tensor, param_tensor, sparse_elbo
-        from ..kernels import Input
+        from ..kernels import Input, flat_under_maps
 
         p_x, x, K_n = self.fdd.p, self.fdd.x, self.fdd.noise
         p_z, z, noise_z = self.u.p, self.u.x, self.u.noise
@@ -244,20 +246,21 @@ class AbstractPseudoObservations(AbstractObservations):
         K_z = M.add(pairwise(measure.kernels[p_z], z), noise_z)
         if not isinstance(K_z, M.KernelDense) or K_z.xg.shape[1] != 1:
             return None
-        plan = self._stream_plan(measure, 1)
+        plan = self._stream_plan(measure, 1, through_maps=True)
         if plan is None:
             return None
-        flat_c, scales_c, _, _ = plan
+        flat_c, scales_c, xm_c, zm_c = plan
         flat_x = coefs_x = xg_x = params_x = None
         if self.method in ("vfe", "fitc"):
-            flat_x, scales_x = measure.kernels[p_x]._flat()
-            if flat_x is None or not flat_x.terms:
+            res = flat_under_maps(measure.kernels[p_x], x)
+            if res is None:
                 return None
-            xg_x = x.scaled(scales_x)
+            flat_x, scales_x, xm_x, _ = res
+            xg_x = xm_x.scaled(scales_x)
             coefs_x, params_x = coef_tensor(flat_x, xg_x), param_tensor(flat_x, xg_x)
         K_z.full_precision = True  # the backward reads L_z^-1 element by element: never the 7-slice factorisation
         coefs_z, ns_z = K_z.grad_params()
-        xg_c, zg_c = x.scaled(scales_c), z.scaled(scales_c)
+        xg_c, zg_c = xm_c.scaled(scales_c), zm_c.scaled(scales_c)
         ybar = (uprank(self.y) - measure.means[p_x].dev(x)).reshape(-1)
         kn = K_n.diag.reshape(-1)
 
@@ -361,7 +364,58 @@ class AbstractPseudoObservations(AbstractObservations):
         for nz in (self.fdd.noise, self.u.noise):
             if isinstance(nz, M.Diagonal):
                 ts.append(nz.diag)
-        return any(isinstance(t, torch.Tensor) and t.requires_grad for t in ts)
+        return any(isinstance(t, torch.Tensor) and t.requires_grad for t in ts) or bool(self._map_grads(measure))
+
+    def _single_kernels(self, measure):
+        """``[(k_z, z, z), (k_zx, z, x), (k_x, x, x)]`` of a problem over one inducing and one observed process with numeric
+        inputs, else None."""
+        from ..kernels import Input
+
+        p_x, x, p_z, z = self.fdd.p, self.fdd.x, self.u.p, self.u.x
+        if not isinstance(x, Input) or not isinstance(z, Input):
+            return None
+        return [(measure.kernels[p_z], z, z), (measure.kernels[p_z, p_x], z, x), (measure.kernels[p_x], x, x)]
+
+    def _mapped(self, measure):
+        """True for a problem over one process whose kernels have input maps: ``generic_grad`` cannot restate those."""
+        ks = self._single_kernels(measure)
+        return ks is not None and any(_maps(k) for k, _, _ in ks)
+
+    def _map_grads(self, measure):
+        """The tensors that require grad behind the input maps of a single-process problem's kernels: the maps' parameters,
+        the hyper-parameters of the kernels inside them and the outputs of transforms (:func:`kernels.map_output_grads`)."""
+        from ..kernels import _grad_tensors, map_output_grads
+
+        out = []
+        for k, a, b in self._single_kernels(measure) or []:
+            if _maps(k):
+                out += _grad_tensors(k) + map_output_grads(k, a, b)
+        return out
+
+    def _compute_uncovered(self, measure):
+        """A single-process problem with input-mapped kernels under grad.  The ELBO takes its analytic route when the kernels
+        resolve under maps; every other result (and the ELBO when they do not) is the no-grad value, attached to the tensors it
+        depends on by ``autograd.no_gradient``: a ``backward()`` through it raises instead of returning a partial gradient."""
+        from ..autograd import no_gradient
+        from ..kernels import _grad_tensors
+
+        key = id(measure)
+        if key not in self._elbo:
+            e = self._elbo_streamed_grad(measure)
+            if e is not None:
+                self._elbo[key] = e
+        # y - m(x) and m(z) themselves: a mean given as a user function hides its parameters in a closure
+        means = (measure.means[self.fdd.p].dev(self.fdd.x), measure.means[self.u.p].dev(self.u.x))
+        ts = _grad_tensors(self.y, self.fdd.x, self.u.x, self.fdd.noise, self.u.noise, means,
+                           [k for k, _, _ in self._single_kernels(measure)]) + self._map_grads(measure)
+        absent = [s for s in (self._K_z, self._mu, self._A, self._elbo) if key not in s]
+        with torch.no_grad():
+            self._compute(measure)
+            values = [M.dense(s[key]) if isinstance(s[key], M.AbstractMatrix) else s[key] for s in absent]
+        route = "a sparse (pseudo-observation) approximation or posterior with input-mapped kernels"
+        for s, v in zip(absent, values):
+            t = no_gradient(route, v, ts)
+            s[key] = M.Dense(t, s[key].origin) if isinstance(s[key], M.AbstractMatrix) else t
 
     def _compute_grad(self, measure):
         from ..generic_grad import sparse_compute_torch
@@ -392,10 +446,12 @@ class AbstractPseudoObservations(AbstractObservations):
 
 
     # -- the two ways to form A = I + W K_n^-1 W^T, prod = W K_n^-1 ybar and the scalars ------------------------------------
-    def _stream_plan(self, measure, batch):
+    def _stream_plan(self, measure, batch, through_maps=False):
         """``(flat, scales, x_input, z_input)`` when the problem can be streamed (one problem, numeric inputs, a symmetric
-        cross-kernel that fits one K1 descriptor), else None.  ``batch``: the number of problems ``K_z`` holds."""
-        from ..kernels import Input, _is_multi
+        cross-kernel that fits one K1 descriptor), else None.  ``batch``: the number of problems ``K_z`` holds.
+        ``through_maps``: also a cross kernel that is one descriptor under input maps, with the mapped inputs (the gradient's
+        rows); the no-grad forward keeps the materialised accumulation for those."""
+        from ..kernels import Input, _is_multi, flat_under_maps
 
         p_x, x, p_z, z = self.fdd.p, self.fdd.x, self.u.p, self.u.x
         if batch != 1 or _is_multi(x) or _is_multi(z) or not isinstance(x, Input) or not isinstance(z, Input):
@@ -403,12 +459,13 @@ class AbstractPseudoObservations(AbstractObservations):
         if x.batch_shape or z.batch_shape:
             return None
         k_zx = measure.kernels[p_z, p_x]
-        if not k_zx.symmetric:
+        if not k_zx.symmetric or (_maps(k_zx) and not through_maps):
             return None
-        flat, scales = k_zx._flat()
-        if flat is None or not flat.terms:
+        res = flat_under_maps(k_zx, z, x)
+        if res is None:
             return None
-        return flat, scales, x, z
+        flat, scales, zm, xm = res
+        return flat, scales, xm, zm
 
     def _accumulate_streamed(self, measure, ch_z, kn3, yb3, flat, scales, x, z):
         """``gpk_sparse_accumulate`` over chunks of data points: O(chunk m + m^2) device memory.  Also returns ``diag K_x``

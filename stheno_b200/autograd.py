@@ -102,8 +102,10 @@ def _alpha_and_G_impl(ch, g):
     Gm = torch.empty(Bn, n_pad, n_pad, dtype=dtype, device=dev)
     kp = ops.round_up(k, 16)
     for b in range(Bn):
-        s = float(g[b].sum())
-        ops.gemm_nt(V[b : b + 1], V[b : b + 1], Gm[b : b + 1], alpha=-0.5 * s, beta=0.0, lower=True)
+        # the weight sum(g_c) scales the product on the device: reading it on the host would make the backward wait for
+        # everything enqueued before it on the stream
+        ops.gemm_nt(V[b : b + 1], V[b : b + 1], Gm[b : b + 1], alpha=-0.5, beta=0.0, lower=True)
+        Gm[b].mul_(g[b].sum())
         A = torch.zeros(1, n_pad, kp, dtype=dtype, device=dev)
         Bm = torch.zeros(1, n_pad, kp, dtype=dtype, device=dev)
         A[0, :n, :k] = (alpha[b] * (0.5 * g[b]).unsqueeze(-1)).t()

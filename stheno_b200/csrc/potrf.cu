@@ -616,8 +616,9 @@ constexpr int64_t NB_OUTER = 512;  // outer panel width
 // event-bracketed launches time single kernels (bench.py's in-situ kernel timing)
 static bool no_lookahead() { return getenv("GPK_NO_LOOKAHEAD") != nullptr; }
 
-// Side stream + events for the look-ahead (one set per process; the library is not re-entrant across host threads
-// for potrf, like the reference's global-state model -- SURVEY 8b "Ownership / threading").
+// Side streams + events for the look-ahead, one set per (host thread, device) (`lookahead()`): concurrent factorisations on
+// different host threads never share them.  Every use forks them from the caller's stream with an event and joins them
+// back before the call returns, so a factorisation is ordered on the caller's stream like any single launch.
 struct Lookahead {
   cudaStream_t side = nullptr;  // the latency-bound chain: leaf factorisations + the rows the next leaf depends on
   cudaStream_t bulk = nullptr;  // the rest of the panel rows (throughput work the chain does not wait for)

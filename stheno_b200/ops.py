@@ -9,6 +9,7 @@ factorised live in a workspace ``W[B, n_pad + extra, n_pad]`` padded to multiple
 """
 import ctypes
 import math
+import threading
 
 import torch
 
@@ -440,7 +441,8 @@ def _potrf(W, n, n_pad, extra, k, well_conditioned=False):
     return Chol(W, n, k, logdet, info)
 
 
-_PRODUCT_SLICES_AUTO = [8]
+#: the slice count of ``product_slices`` for the calling host thread (8 outside a ``with`` block)
+_PRODUCT_SLICES = threading.local()
 
 
 class product_slices:
@@ -449,17 +451,18 @@ class product_slices:
     solve and one big product, 1.3x faster with 7 slices.  Measured against torch fp64 autograd
     (``tests/test_logpdf_grad_paths.py``), 7-slice solves and products on an 8-slice factor keep the gradients within a
     small factor of native fp64's error from noise 1e-2 to 1e-6 of the variance; a 7-slice FACTOR does not (up to 45x
-    at 1e-2), so a factorisation whose gradient is taken is asked for with ``full_precision``."""
+    at 1e-2), so a factorisation whose gradient is taken is asked for with ``full_precision``.  The setting belongs to the
+    host thread that enters the block: calls made meanwhile on other threads keep their own."""
 
     def __init__(self, slices):
         self.slices = int(slices)
 
     def __enter__(self):
-        self.prev = _PRODUCT_SLICES_AUTO[0]
-        _PRODUCT_SLICES_AUTO[0] = self.slices
+        self.prev = getattr(_PRODUCT_SLICES, "auto", 8)
+        _PRODUCT_SLICES.auto = self.slices
 
     def __exit__(self, *exc):
-        _PRODUCT_SLICES_AUTO[0] = self.prev
+        _PRODUCT_SLICES.auto = self.prev
 
 
 def _oz_slices(well_conditioned=False):
@@ -478,7 +481,7 @@ def _oz_slices(well_conditioned=False):
 
     mode = getattr(_Bns, "precision", "auto")
     if mode == "auto":
-        return 7 if well_conditioned else _PRODUCT_SLICES_AUTO[0]
+        return 7 if well_conditioned else getattr(_PRODUCT_SLICES, "auto", 8)
     return {"int8x5": 5, "int8x6": 6, "int8x7": 7, "int8x8": 8}.get(mode, 0)
 
 
@@ -498,27 +501,41 @@ def _well_conditioned(flat, noise_scalar, noise_vec, jitter):
     return diag >= 1e-3 * max(scale, 1e-300)
 
 
-#: per-device scratch of the int8-slice emulation, shared by every call on the device (they are stream-ordered)
+#: scratch of the int8-slice emulation per (device, stream): the calls on one stream are ordered by it, calls on two streams
+#: may run at the same time, so each stream has its own
 _OZ_SCRATCH = {}
 _OZ_SCRATCH_MAX_BYTES = 8 << 30
 
 
 def _emulation(dtype, device, need, well_conditioned=False):
     """The trailing ``(slices, ws, ws_bytes)`` arguments of an fp64 entry point (none for fp32): ``B.precision``'s slice count
-    (:func:`_oz_slices`) and ``device``'s scratch, grown on demand to ``need(lib, slices)`` bytes -- the library's size query
-    for the call -- and capped (larger requests stay on the fp64 tensor cores).  ``(0, NULL, 0)`` when the slice count or
-    the need is 0: the call runs on the fp64 tensor cores."""
+    (:func:`_oz_slices`) and the scratch of the current stream, grown on demand to ``need(lib, slices)`` bytes -- the library's
+    size query for the call -- and capped (larger requests stay on the fp64 tensor cores).  ``(0, NULL, 0)`` when the slice
+    count or the need is 0: the call runs on the fp64 tensor cores.  The scratch is allocated on the stream that uses it, so
+    the buffer a growth replaces returns to that stream's pool, reused only by work ordered after the calls that read it."""
     if dtype != torch.float64:
         return ()
     slices = _oz_slices(well_conditioned)
     need_bytes = min(int(need(_lib.load(), slices)), _OZ_SCRATCH_MAX_BYTES) if slices else 0
     if not need_bytes:
         return 0, None, 0
-    key = torch.device(device).index or 0
+    stream = torch.cuda.current_stream(device)
+    key = (stream.device_index, stream.cuda_stream)
     buf = _OZ_SCRATCH.get(key)
     if buf is None or buf.numel() < need_bytes:
-        buf = _OZ_SCRATCH[key] = _aligned_bytes(max(need_bytes, 64 << 20), torch.device("cuda", key))
+        buf = _OZ_SCRATCH[key] = _aligned_bytes(max(need_bytes, 64 << 20), stream.device)
     return slices, _ptr(buf), buf.numel()
+
+
+def release_scratch(stream=None):
+    """Drop the emulation scratch of ``stream`` (a ``torch.cuda.Stream``; every stream's when None), for a stream that will not
+    run emulated calls again.  Safe while work that uses it is still queued: the buffer goes back to the pool of the stream it
+    was allocated on and is reused only by work ordered after that; ``torch.cuda.empty_cache()`` then returns it to the
+    device."""
+    if stream is None:
+        _OZ_SCRATCH.clear()
+    else:
+        _OZ_SCRATCH.pop((stream.device_index, stream.cuda_stream), None)
 
 
 def _aligned_bytes(nbytes, device, align=1024):

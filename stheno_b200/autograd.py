@@ -271,95 +271,16 @@ def no_gradient(route, value, inputs):
 # L = chol(K_z + eps I), W = L^-1 K_zx (columns w_i), kappa_i = K_n' (:311-313), A = I + W diag(1/kappa) W^T, s = A^-1 prod.
 # gpk_sparse_rows_bwd gives the per-point gradients and g_i = dE/dw_i; E depends on W only through W^T W, so H = sum_i g_i w_i^T
 # is symmetric and   dE/dK_zx[:, i] = L^-T g_i,   dE/dK_z = -1/2 L^-T H L^-1.
+# K_z = [k(u_q, u_q')], K_zx = [k(u_q, f_p)] and diag K_x = [diag k(f_p)] are assembled from blocks, one per pair of
+# processes (one of each over one inducing and one observed process): only forming the rows and contracting the gradients
+# go block by block.  The forward factors K_z with the lower blocks only, so a block below the diagonal receives
+# dE/dK_z[q, q'] + dE/dK_z[q', q]^T = 2 GK[q, q'] (GK = dE/dK_z is symmetric).
 class SparseElboSpec:
-    """What one sparse ELBO needs beyond its tensor inputs: the method, the flat kernels of ``K_z`` (``flat_z``), of the cross
-    kernel (``flat_c``) and of ``k_x`` (``flat_x``, None for DTC), the chunk, and ``fwd()``, which runs the launches of the
-    no-grad path and returns ``(ch_z, ch_A, s, kdiag, elbo)`` (``kdiag`` None where that path does not stream: the backward
-    then forms ``diag K_x`` itself)."""
-
-    def __init__(self, method, flat_z, flat_c, flat_x, chunk, fwd):
-        self.method, self.flat_z, self.flat_c, self.flat_x, self.chunk, self.fwd = method, flat_z, flat_c, flat_x, chunk, fwd
-
-
-class _SparseElbo(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, spec, coefs_z, zg_z, ns_z, nv_z, coefs_c, xg_c, zg_c, coefs_x, xg_x, kn, ybar, params_z, params_c,
-                params_x):
-        ch_z, ch_A, s, kdiag, elbo = spec.fwd()
-        ctx.spec, ctx.ch_z, ctx.ch_A, ctx.s, ctx.kdiag = spec, ch_z, ch_A, s, kdiag
-        ctx.zg_z, ctx.xg_c, ctx.zg_c = zg_z.detach().contiguous(), xg_c.detach().contiguous(), zg_c.detach().contiguous()
-        ctx.xg_x = None if xg_x is None else xg_x.detach().contiguous()
-        ctx.kn, ctx.ybar = kn.detach(), ybar.detach()
-        ctx.nv_shape = None if nv_z is None else nv_z.shape
-        return elbo
-
-    @staticmethod
-    def backward(ctx, g):
-        spec, ch_z = ctx.spec, ctx.ch_z
-        (_, want_coefs_z, want_zg_z, want_ns, want_nv, want_coefs_c, want_xg_c, want_zg_c, want_coefs_x, want_xg_x, _,
-         _, want_params_z, want_params_c, want_params_x) = ctx.needs_input_grad
-        dt, dev, m = ch_z.dtype, ch_z.device, ch_z.n
-        want_K = want_coefs_z or want_zg_z or want_ns or want_nv or want_params_z
-        ts_c = torch.zeros(1, _lib.GPK_MAX_TERMS, dtype=dt, device=dev) if want_coefs_c else None
-        g_xc = torch.zeros_like(ctx.xg_c) if want_xg_c else None
-        g_zc = torch.zeros_like(ctx.zg_c) if want_zg_c else None
-        ps_c = _param_buf(want_params_c, 1, ctx.xg_c)
-        kdiag = ctx.kdiag
-        if kdiag is None and spec.method != "dtc":  # the materialised forward (input-mapped kernels) did not keep diag K_x
-            kdiag = ops.kernel_diag(spec.flat_x, ctx.xg_x)[0]
-        g_kn, g_kd, g_y, H = ops.sparse_elbo_bwd(
-            spec.flat_c, ctx.xg_c, ctx.zg_c, ch_z, ctx.ch_A, ctx.s, kdiag, ctx.kn, ctx.ybar, spec.method, spec.chunk,
-            want_H=want_K, want_cross=want_coefs_c or want_xg_c or want_zg_c or want_params_c, term_sum=ts_c, grad_xg=g_xc,
-            grad_zg=g_zc, param_sum=ps_c)
-        grads = dict(kn=g_kn, ybar=g_y, coefs_c=None if ts_c is None else ts_c[0, : len(spec.flat_c.terms)], xg_c=g_xc,
-                     zg_c=g_zc, params_c=_param_grad(spec.flat_c, ps_c))
-        if want_K:
-            # dE/dK_z = -1/2 L^-T H L^-1: two transposed solves with a transpose between them
-            m_pad = ch_z.n_pad
-            ch_z.solve_many_rows_t_(H)
-            GK = ops.transpose(H, m_pad, m_pad)
-            del H
-            ch_z.solve_many_rows_t_(GK)
-            GK.mul_(-0.5)
-            ops.symmetrize_(GK, m_pad)
-            ps_z = _param_buf(want_params_z, 1, ctx.zg_z)
-            term_sum, g_zz, diag = _bwd_kernel(spec.flat_z, ctx.zg_z, GK, m, ps_z)
-            del GK
-            grads.update(coefs_z=term_sum[0, : len(spec.flat_z.terms)] if want_coefs_z else None, zg_z=g_zz if want_zg_z else None,
-                         ns=diag.sum() if want_ns else None, nv=diag.reshape(ctx.nv_shape) if want_nv else None,
-                         params_z=_param_grad(spec.flat_z, ps_z))
-        if want_coefs_x or want_xg_x or want_params_x:
-            fx = spec.flat_x
-            ts_x = torch.zeros(1, _lib.GPK_MAX_TERMS, dtype=dt, device=dev) if want_coefs_x else None
-            g_xx = torch.zeros_like(ctx.xg_x) if want_xg_x else None
-            ps_x = _param_buf(want_params_x, 1, ctx.xg_x)
-            ops.kernel_cross_bwd(fx, ctx.xg_x, ctx.xg_x, gdiag=g_kd.unsqueeze(0), term_sum=ts_x, grad_xsg=g_xx, param_sum=ps_x)
-            grads.update(coefs_x=None if ts_x is None else ts_x[0, : len(fx.terms)], xg_x=g_xx, params_x=_param_grad(fx, ps_x))
-        order = ("coefs_z", "zg_z", "ns", "nv", "coefs_c", "xg_c", "zg_c", "coefs_x", "xg_x", "kn", "ybar", "params_z",
-                 "params_c", "params_x")
-        return (None,) + tuple(None if grads.get(k) is None else g * grads[k] for k in order)
-
-
-def sparse_elbo(spec, coefs_z, zg_z, ns_z, nv_z, coefs_c, xg_c, zg_c, coefs_x, xg_x, kn, ybar, params_z=None, params_c=None,
-                params_x=None):
-    """The ELBO ``spec.fwd()`` computes, differentiable w.r.t. the coefficients and pre-stretched inputs of ``K_z``'s kernel
-    (``coefs_z``, ``zg_z``), its scalar and vector noise (``ns_z``, ``nv_z``), the cross kernel's (``coefs_c``, ``xg_c``, ``zg_c``)
-    and ``k_x``'s (``coefs_x``, ``xg_x``; None for DTC), the observation noise ``kn [n]``, ``ybar [n]`` and the three kernels'
-    shape parameters (``params_z``, ``params_c``, ``params_x``: :func:`param_tensor`)."""
-    return _SparseElbo.apply(spec, coefs_z, zg_z, ns_z, nv_z, coefs_c, xg_c, zg_c, coefs_x, xg_x, kn, ybar, params_z, params_c,
-                             params_x)
-
-
-# ---- the sparse ELBO over several processes (PseudoObs with tuples of FDDs) ---------------------------------------------------
-#
-# The same math on the assembled K_z = [k(u_q, u_q')], K_zx = [k(u_q, f_p)], diag K_x = [diag k(f_p)]: only forming the rows
-# and contracting the gradients go block by block.  The forward factors K_z with the lower blocks only, so a block below the
-# diagonal receives dE/dK_z[q, q'] + dE/dK_z[q', q]^T = 2 GK[q, q'] (GK = dE/dK_z is symmetric).
-class MultiSparseElboSpec:
-    """What one multi-output sparse ELBO needs beyond its tensor inputs: the method, ``z_sizes`` (``m_q``) and ``x_sizes``
-    (``n_p``); the nonzero blocks as flat kernels: ``kz`` ``[(q, q', flat)]`` with ``q' <= q``, ``cross`` ``[(p, q, flat)]``
+    """What one sparse ELBO needs beyond its tensor inputs: the method, ``z_sizes`` (``m_q``) and ``x_sizes`` (``n_p``);
+    the nonzero blocks as flat kernels: ``kz`` ``[(q, q', flat)]`` with ``q' <= q``, ``cross`` ``[(p, q, flat)]``
     (``k(f_p, u_q)``) and ``kx`` ``[(p, flat)]`` (``k(f_p)``, empty for DTC); the chunk; and ``fwd()``, which runs the
-    launches of the no-grad path and returns ``(ch_z, ch_A, s, elbo)``."""
+    launches of the no-grad path and returns ``(ch_z, ch_A, s, kdiag, elbo)`` (``kdiag``: the ``diag K_x`` that path
+    streamed, else None: the backward then forms it from the ``kx`` blocks)."""
 
     def __init__(self, method, z_sizes, x_sizes, kz, cross, kx, chunk, fwd):
         self.method, self.z_sizes, self.x_sizes, self.chunk, self.fwd = method, list(z_sizes), list(x_sizes), chunk, fwd
@@ -368,15 +289,15 @@ class MultiSparseElboSpec:
         self.x_off = [sum(self.x_sizes[:p]) for p in range(len(self.x_sizes))]
 
 
-class _MultiSparseElbo(torch.autograd.Function):
+class _SparseElbo(torch.autograd.Function):
     """Inputs after ``spec``: per ``kz`` block ``(coefs, zg_q, zg_q' or None on the diagonal, params)``, the inducing noise
     ``nz [m]`` or None, per ``cross`` block ``(coefs, xg_p, zg_q, params)``, per ``kx`` block ``(coefs, xg_p, params)``, then
     ``kn [n]`` and ``ybar [n]``."""
 
     @staticmethod
     def forward(ctx, spec, *ts):
-        ch_z, ch_A, s, elbo = spec.fwd()
-        ctx.spec, ctx.ch_z, ctx.ch_A, ctx.s = spec, ch_z, ch_A, s
+        ch_z, ch_A, s, kdiag, elbo = spec.fwd()
+        ctx.spec, ctx.ch_z, ctx.ch_A, ctx.s, ctx.kdiag = spec, ch_z, ch_A, s, kdiag
         ctx.ts = [None if t is None else t.detach() for t in ts]
         return elbo
 
@@ -397,8 +318,8 @@ class _MultiSparseElbo(torch.autograd.Function):
             return torch.zeros(1, _lib.GPK_MAX_TERMS, dtype=dt, device=dev) if nig[i] else None
 
         # kdiag = diag K_x over all processes (VFE / FITC): what the forward's rows read
-        kdiag = None
-        if spec.method != "dtc":
+        kdiag = ctx.kdiag
+        if kdiag is None and spec.method != "dtc":
             kdiag = torch.zeros(sum(spec.x_sizes), dtype=dt, device=dev)
             for b, (p, flat) in enumerate(spec.kx):
                 a = spec.x_off[p]
@@ -415,8 +336,8 @@ class _MultiSparseElbo(torch.autograd.Function):
                                  param_sum=_param_buf(nig[k + 3], 1, xg))
             procs[p][1].append(blk)
             outs.append((k, flat, blk))
-        g_kn, g_kd, g_y, H = ops.sparse_elbo_bwd_multi(procs, ch_z, ctx.ch_A, ctx.s, kdiag, ts[i_kn], ts[i_kn + 1],
-                                                       spec.method, spec.chunk, want_H=want_K, want_cross=want_cross)
+        g_kn, g_kd, g_y, H = ops.sparse_elbo_bwd(procs, ch_z, ctx.ch_A, ctx.s, kdiag, ts[i_kn], ts[i_kn + 1], spec.method,
+                                                 spec.chunk, want_H=want_K, want_cross=want_cross)
         grads[i_kn], grads[i_kn + 1] = g_kn, g_y
         for k, flat, blk in outs:
             grads[k] = None if blk.term_sum is None else blk.term_sum[0, : len(flat.terms)]
@@ -472,13 +393,12 @@ class _MultiSparseElbo(torch.autograd.Function):
         return (None,) + tuple(None if (gr is None or not w) else g * gr for gr, w in zip(grads, nig))
 
 
-def multi_sparse_elbo(spec, kz, nz, cross, kx, kn, ybar):
-    """The ELBO ``spec.fwd()`` computes for a problem over several processes, differentiable w.r.t. every block's coefficients,
-    pre-stretched inputs and shape parameters (``kz``, ``cross``, ``kx``: one tuple of tensors per block of ``spec``, in
-    :class:`_MultiSparseElbo`'s order), the inducing noise ``nz [m]`` (None: none), the observation noise ``kn [n]`` and
-    ``ybar [n]``."""
+def sparse_elbo(spec, kz, nz, cross, kx, kn, ybar):
+    """The ELBO ``spec.fwd()`` computes, differentiable w.r.t. every block's coefficients, pre-stretched inputs and shape
+    parameters (``kz``, ``cross``, ``kx``: one tuple of tensors per block of ``spec``, in :class:`_SparseElbo`'s order), the
+    inducing noise ``nz [m]`` (None: none), the observation noise ``kn [n]`` and ``ybar [n]``."""
     flat_ts = [t for blk in kz for t in blk] + [nz] + [t for blk in cross for t in blk] + [t for blk in kx for t in blk]
-    return _MultiSparseElbo.apply(spec, *flat_ts, kn, ybar)
+    return _SparseElbo.apply(spec, *flat_ts, kn, ybar)
 
 
 # ---- sparse posterior predictions in the test inputs ------------------------------------------------------------------------

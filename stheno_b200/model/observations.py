@@ -130,9 +130,7 @@ class AbstractPseudoObservations(AbstractObservations):
 
     def elbo(self, measure):
         if id(measure) not in self._elbo and self._wants_grad(measure):
-            e = self._elbo_streamed_grad(measure)
-            if e is None:
-                e = self._elbo_multi_grad(measure)
+            e = self._elbo_grad(measure)
             if e is not None:
                 self._elbo[id(measure)] = e
         e = self._get(self._elbo, measure)
@@ -227,62 +225,15 @@ class AbstractPseudoObservations(AbstractObservations):
         elbo = -0.5 * (det_part + iqf_part + trace_part)
         return A, ch_A, sol, elbo, kd
 
-    # -- analytic streamed gradient (autograd.sparse_elbo): the ELBO under grad of one problem on the GPU ---------------------
-    def _elbo_streamed_grad(self, measure):
-        """The ELBO with the analytic backward of ``autograd.sparse_elbo``, or None when the problem is not covered: it needs
-        one problem of numeric inputs, ``k_z``, a symmetric ``k_zx`` and ``k_x`` that are each one flat descriptor under input
-        maps (:func:`kernels.flat_under_maps`), Diagonal noise, Zero or Diagonal inducing noise, and data on a CUDA device.
-        The backward streams the rows of ``k_zx`` at the mapped points; the forward runs the no-grad launches (for mapped
-        kernels the materialised accumulation)."""
+    # -- analytic streamed gradient (autograd.sparse_elbo): the ELBO under grad on the GPU ----------------------------------
+    def _elbo_grad(self, measure):
+        """The ELBO with the analytic backward of ``autograd.sparse_elbo``, or None when the problem is not covered: every
+        block ``k(u_q, u_q')``, ``k(u_q, f_p)`` (also symmetric) and, for VFE / FITC, ``k(f_p)`` has to flatten to one
+        descriptor or be zero (over one inducing and one observed process, also under input maps: :func:`_flat_block`), no
+        input may have a batch dimension, the noise has to be Diagonal and the inducing noise Zero or Diagonal, and the data
+        have to be on a CUDA device.  The forward runs the launches of the no-grad route."""
         from ..autograd import SparseElboSpec, coef_tensor, param_tensor, sparse_elbo
-        from ..kernels import Input, flat_under_maps
 
-        p_x, x, K_n = self.fdd.p, self.fdd.x, self.fdd.noise
-        p_z, z, noise_z = self.u.p, self.u.x, self.u.noise
-        if not isinstance(K_n, M.Diagonal) or not isinstance(noise_z, (M.Zero, M.Diagonal)):
-            return None
-        if not isinstance(x, Input) or not isinstance(z, Input) or not x.t.is_cuda:
-            return None
-        K_z = M.add(pairwise(measure.kernels[p_z], z), noise_z)
-        if not isinstance(K_z, M.KernelDense) or K_z.xg.shape[1] != 1:
-            return None
-        plan = self._stream_plan(measure, 1, through_maps=True)
-        if plan is None:
-            return None
-        flat_c, scales_c, xm_c, zm_c = plan
-        flat_x = coefs_x = xg_x = params_x = None
-        if self.method in ("vfe", "fitc"):
-            res = flat_under_maps(measure.kernels[p_x], x)
-            if res is None:
-                return None
-            flat_x, scales_x, xm_x, _ = res
-            xg_x = xm_x.scaled(scales_x)
-            coefs_x, params_x = coef_tensor(flat_x, xg_x), param_tensor(flat_x, xg_x)
-        K_z.full_precision = True  # the backward reads L_z^-1 element by element: never the 7-slice factorisation
-        coefs_z, ns_z = K_z.grad_params()
-        xg_c, zg_c = xm_c.scaled(scales_c), zm_c.scaled(scales_c)
-        ybar = (uprank(self.y) - measure.means[p_x].dev(x)).reshape(-1)
-        kn = K_n.diag.reshape(-1)
-
-        def fwd():
-            ch_z = K_z.chol()
-            _, ch_A, sol, elbo, kd = self._elbo_from_factor(measure, ch_z, kn.reshape(1, -1), ybar.reshape(1, -1, 1))
-            return ch_z, ch_A, sol[0, 0], kd, elbo[0]
-
-        spec = SparseElboSpec(self.method, K_z.flat, flat_c, flat_x, B.sparse_chunk, fwd)
-        return sparse_elbo(spec, coefs_z, K_z.xg, ns_z, K_z.noise_vec, coef_tensor(flat_c, xg_c), xg_c, zg_c, coefs_x, xg_x,
-                           kn, ybar, param_tensor(K_z.flat, K_z.xg), param_tensor(flat_c, xg_c), params_x)
-
-    def _elbo_multi_grad(self, measure):
-        """The ELBO with the analytic backward of ``autograd.multi_sparse_elbo`` when the inducing points and / or the
-        observations span several processes (``self.u.x`` or ``self.fdd.x`` a tuple of FDDs), or None when the problem is not
-        covered: every block ``k(u_q, u_q')``, ``k(u_q, f_p)`` (also symmetric) and, for VFE / FITC, ``k(f_p)`` has to flatten to
-        one descriptor or be zero, no input may have a batch dimension, the noise has to be Diagonal and the inducing noise
-        Zero or Diagonal, and the data have to be on a CUDA device."""
-        from ..autograd import MultiSparseElboSpec, coef_tensor, multi_sparse_elbo, param_tensor
-
-        if not isinstance(self.u.x, tuple) and not isinstance(self.fdd.x, tuple):
-            return None
         K_n, noise_z = self.fdd.noise, self.u.noise
         if not isinstance(K_n, M.Diagonal) or not isinstance(noise_z, (M.Zero, M.Diagonal)):
             return None
@@ -291,34 +242,38 @@ class AbstractPseudoObservations(AbstractObservations):
             return None
         if any(v.batch_shape or not v.t.is_cuda for _, v in us + fs):
             return None
+        maps = len(us) == 1 and len(fs) == 1
         kz, cross, kx = [], [], []
         spec_kz, spec_cross, spec_kx = [], [], []
         for q, (pq, zq) in enumerate(us):
             for q2, (pq2, zq2) in enumerate(us):
-                flat, scales = measure.kernels[pq, pq2]._flat()
-                if flat is None:
+                blk = _flat_block(measure.kernels[pq, pq2], zq, None if q2 == q else zq2, maps)
+                if blk is None:
                     return None
+                flat, scales, zm, zm2 = blk
                 if q2 <= q and flat.terms:
-                    zg = zq.scaled(scales)
-                    zg2 = None if q2 == q else zq2.scaled(scales)
+                    zg = zm.scaled(scales)
+                    zg2 = None if q2 == q else zm2.scaled(scales)
                     spec_kz.append((q, q2, flat))
                     kz.append((coef_tensor(flat, zg), zg, zg2, param_tensor(flat, zg)))
         for p, (pp, xp) in enumerate(fs):
             for q, (pq, zq) in enumerate(us):
                 k = measure.kernels[pq, pp]
-                flat, scales = k._flat()
-                if flat is None or not k.symmetric:
+                blk = _flat_block(k, zq, xp, maps) if k.symmetric else None
+                if blk is None:
                     return None
+                flat, scales, zm, xm = blk
                 if flat.terms:
-                    xg = xp.scaled(scales)
+                    xg = xm.scaled(scales)
                     spec_cross.append((p, q, flat))
-                    cross.append((coef_tensor(flat, xg), xg, zq.scaled(scales), param_tensor(flat, xg)))
+                    cross.append((coef_tensor(flat, xg), xg, zm.scaled(scales), param_tensor(flat, xg)))
             if self.method in ("vfe", "fitc"):
-                flat, scales = measure.kernels[pp]._flat()
-                if flat is None:
+                blk = _flat_block(measure.kernels[pp], xp, None, maps)
+                if blk is None:
                     return None
+                flat, scales, xm, _ = blk
                 if flat.terms:
-                    xg = xp.scaled(scales)
+                    xg = xm.scaled(scales)
                     spec_kx.append((p, flat))
                     kx.append((coef_tensor(flat, xg), xg, param_tensor(flat, xg)))
         p_x, x, p_z, z = self.fdd.p, self.fdd.x, self.u.p, self.u.x
@@ -327,18 +282,18 @@ class AbstractPseudoObservations(AbstractObservations):
         nz = noise_z.diag.reshape(-1) if isinstance(noise_z, M.Diagonal) else None
 
         def fwd():
-            # the launches of the no-grad route (_compute): the BlockDense factor of K_z, the materialised accumulation
+            # the launches of the no-grad route (_compute): the factor of K_z, the streamed or materialised accumulation
             K_z = M._densify(M.add(pairwise(measure.kernels[p_z], z), noise_z))
             if isinstance(K_z, M.KernelDense):
-                K_z.full_precision = True  # one inducing process: never the 7-slice factorisation, as on the single route
+                K_z.full_precision = True  # the backward reads L_z^-1 element by element: never the 7-slice factorisation
             ch_z = K_z.chol()
-            _, ch_A, sol, elbo, _ = self._elbo_from_factor(measure, ch_z, kn.reshape(1, -1), ybar.reshape(1, -1, 1))
-            return ch_z, ch_A, sol[0, 0], elbo[0]
+            del K_z  # under input maps it holds mapped points of its own: free them before the accumulation's peak
+            _, ch_A, sol, elbo, kd = self._elbo_from_factor(measure, ch_z, kn.reshape(1, -1), ybar.reshape(1, -1, 1))
+            return ch_z, ch_A, sol[0, 0], kd, elbo[0]
 
-        spec = MultiSparseElboSpec(self.method, [v.n for _, v in us], [v.n for _, v in fs], spec_kz, spec_cross, spec_kx,
-                                   B.sparse_chunk, fwd)
-        return multi_sparse_elbo(spec, kz, nz, cross, kx, kn, ybar)
-
+        spec = SparseElboSpec(self.method, [v.n for _, v in us], [v.n for _, v in fs], spec_kz, spec_cross, spec_kx,
+                              B.sparse_chunk, fwd)
+        return sparse_elbo(spec, kz, nz, cross, kx, kn, ybar)
 
     # -- differentiable route (generic_grad.py): used only when something that feeds the ELBO requires grad -----------------
     def _wants_grad(self, measure):
@@ -401,7 +356,7 @@ class AbstractPseudoObservations(AbstractObservations):
 
         key = id(measure)
         if key not in self._elbo:
-            e = self._elbo_streamed_grad(measure)
+            e = self._elbo_grad(measure)
             if e is not None:
                 self._elbo[key] = e
         # y - m(x) and m(z) themselves: a mean given as a user function hides its parameters in a closure
@@ -446,12 +401,11 @@ class AbstractPseudoObservations(AbstractObservations):
 
 
     # -- the two ways to form A = I + W K_n^-1 W^T, prod = W K_n^-1 ybar and the scalars ------------------------------------
-    def _stream_plan(self, measure, batch, through_maps=False):
+    def _stream_plan(self, measure, batch):
         """``(flat, scales, x_input, z_input)`` when the problem can be streamed (one problem, numeric inputs, a symmetric
-        cross-kernel that fits one K1 descriptor), else None.  ``batch``: the number of problems ``K_z`` holds.
-        ``through_maps``: also a cross kernel that is one descriptor under input maps, with the mapped inputs (the gradient's
-        rows); the no-grad forward keeps the materialised accumulation for those."""
-        from ..kernels import Input, _is_multi, flat_under_maps
+        cross-kernel without input maps that fits one K1 descriptor), else None.  ``batch``: the number of problems ``K_z``
+        holds."""
+        from ..kernels import Input, _is_multi
 
         p_x, x, p_z, z = self.fdd.p, self.fdd.x, self.u.p, self.u.x
         if batch != 1 or _is_multi(x) or _is_multi(z) or not isinstance(x, Input) or not isinstance(z, Input):
@@ -459,13 +413,12 @@ class AbstractPseudoObservations(AbstractObservations):
         if x.batch_shape or z.batch_shape:
             return None
         k_zx = measure.kernels[p_z, p_x]
-        if not k_zx.symmetric or (_maps(k_zx) and not through_maps):
+        if not k_zx.symmetric or _maps(k_zx):
             return None
-        res = flat_under_maps(k_zx, z, x)
-        if res is None:
+        flat, scales = k_zx._flat()
+        if flat is None or not flat.terms:
             return None
-        flat, scales, zm, xm = res
-        return flat, scales, xm, zm
+        return flat, scales, x, z
 
     def _accumulate_streamed(self, measure, ch_z, kn3, yb3, flat, scales, x, z):
         """``gpk_sparse_accumulate`` over chunks of data points: O(chunk m + m^2) device memory.  Also returns ``diag K_x``
@@ -514,6 +467,19 @@ class AbstractPseudoObservations(AbstractObservations):
         det_kn = torch.log(2 * B.pi * kn3).sum(-1)
         yky = (yb3[..., 0] ** 2 / kn3).sum(-1)
         return A, prod, det_kn, yky, trace_part
+
+def _flat_block(k, a, b, maps):
+    """``k(a, b)`` (``b`` None: the square ``k(a, a)``) for the analytic ELBO as ``(flat, scales, am, bm)``: the descriptor
+    and length scales of :meth:`Kernel._flat` (no terms: a zero block) and the points it reads (``bm is am`` for the square
+    form), or None when the block has no analytic route.  A kernel with input maps is its inner descriptor at the mapped
+    points (:func:`kernels.flat_under_maps`), and only where ``maps`` allows it."""
+    from ..kernels import flat_under_maps
+
+    if _maps(k):
+        return flat_under_maps(k, a, b) if maps else None
+    flat, scales = k._flat()
+    return None if flat is None else (flat, scales, a, a if b is None else b)
+
 
 def _parts(fdd):
     """``[(process, Input), ...]`` of an FDD over one process or over a tuple of single-process FDDs, else None."""

@@ -771,74 +771,9 @@ class SparseAccumulator:
         check(rc, "gpk_sparse_accumulate")
 
 
-def sparse_elbo_bwd(flat, xg, zg, ch_z, ch_A, s, kdiag, kn, ybar, method, chunk, want_H=True, want_cross=True,
-                    term_sum=None, grad_xg=None, grad_zg=None, param_sum=None):
-    """Backward of the ELBO :class:`SparseAccumulator` streams, over the same chunks of data points.  ``flat``, ``xg [G, 1, n, d]``,
-    ``zg [G, 1, m, d]``: the cross kernel and its pre-stretched inputs; ``ch_z``: factor of ``K_z``; ``ch_A``: factor of
-    ``A = I + W K_n^-1 W^T``; ``s = A^-1 prod [m]``; ``kdiag`` (None for DTC), ``kn``, ``ybar``: ``[n]``.
-
-    Per chunk: K1 rows and the solve give ``W_c`` (the forward's launches), ``U_c = W_c A^-1``, and ``gpk_sparse_rows_bwd`` turns
-    ``U_c`` into ``G_c`` (rows ``dE/dw_i``) and writes the per-point gradients.  With ``want_H``, ``H += G_c^T W_c`` on the lower
-    tiles (mirrored after the last chunk; ``dE/dK_z = -1/2 L^-T H L^-1``).  With ``want_cross``, the transposed solve turns
-    ``G_c`` into rows ``dE/dk(z, x_i)`` and the rectangular K1-backward adds to ``term_sum``, ``grad_xg``, ``grad_zg`` and
-    ``param_sum`` (each optional, accumulated).  Returns ``(g_kn [n], g_kd [n] or None, g_ybar [n], H [1, m_pad, m_pad] or None)``.  Device memory:
-    four ``chunk x m_pad`` buffers and three ``m_pad x m_pad`` ones."""
-    _require_cuda(xg, zg, kdiag, kn, ybar, term_sum, grad_xg, grad_zg, param_sum)
-    meth = SPARSE_METHOD[method]
-    m, m_pad, dt, dev = ch_z.n, ch_z.n_pad, ch_z.dtype, ch_z.device
-    n, d = xg.shape[2], xg.shape[3]
-    zg = zg.contiguous()
-    V = torch.zeros(1, m_pad, m_pad, dtype=dt, device=dev)
-    V.diagonal(dim1=1, dim2=2).fill_(1.0)
-    ch_A.solve_rows_(V)  # V = L_A^-T, A^-1 = V V^T (the identity on the padding)
-    Ainv = gemm_nt(V, V)
-    del V
-    sp = torch.zeros(m_pad, dtype=dt, device=dev)
-    sp[:m] = s
-    g_kn = torch.empty(n, dtype=dt, device=dev)
-    g_ybar = torch.empty(n, dtype=dt, device=dev)
-    g_kd = torch.empty(n, dtype=dt, device=dev) if meth != 2 else None
-    kdiag, kn, ybar = [None if t is None else t.contiguous() for t in (kdiag, kn, ybar)]
-    H = torch.zeros(1, m_pad, m_pad, dtype=dt, device=dev) if want_H else None
-    rows = round_up(min(int(chunk), n))
-    Wb = torch.empty(1, rows, m_pad, dtype=dt, device=dev)
-    Ub = torch.empty(1, rows, m_pad, dtype=dt, device=dev)
-    if want_H:
-        WTb = torch.empty(1, m_pad, rows, dtype=dt, device=dev)
-        GTb = torch.empty(1, m_pad, rows, dtype=dt, device=dev)
-    fn = _fn("gpk_sparse_rows_bwd", dt)
-    for a in range(0, n, int(chunk)):
-        b = min(n, a + int(chunk))
-        c, cp = b - a, round_up(b - a)
-        xc = xg[:, :, a:b].contiguous()
-        Wc, Uc = Wb[:, :cp], Ub[:, :cp]
-        _km_launch(flat, xc, zg, c, m, d, KM_PAD_ZERO, 0.0, None, 0.0, Wc, Wc.stride(1), Wc.stride(0), 1)
-        ch_z.solve_rows_(Wc)
-        q = row_dot_sq(Wc, c, m_pad, None)[1] if meth != 2 else None
-        gemm_nt(Wc, Ainv, Uc)
-        rc = fn(c, m_pad, _ptr(Wc), Wc.stride(1), _ptr(Uc), Uc.stride(1), _ptr(sp), _ptr(q),
-                _ptr(None if kdiag is None else kdiag[a:b]), _ptr(kn[a:b]), _ptr(ybar[a:b]), meth, _ptr(g_kn[a:b]),
-                _ptr(None if g_kd is None else g_kd[a:b]), _ptr(g_ybar[a:b]), _stream())
-        check(rc, "gpk_sparse_rows_bwd")
-        if want_H:
-            WT, GT = WTb[:, :, :cp], GTb[:, :, :cp]
-            transpose(Wc, cp, m_pad, out=WT)
-            transpose(Uc, cp, m_pad, out=GT)
-            gemm_nt(GT, WT, H, beta=1.0, lower=True)
-        if want_cross:
-            ch_z.solve_many_rows_t_(Uc)
-            gx = torch.zeros_like(xc) if grad_xg is not None else None
-            kernel_cross_bwd(flat, xc, zg, W=Uc, term_sum=term_sum, grad_xsg=gx, grad_xg=grad_zg, param_sum=param_sum)
-            if gx is not None:
-                grad_xg[:, :, a:b] += gx
-    if want_H:
-        symmetrize_(H, m_pad)
-    return g_kn, g_kd, g_ybar, H
-
-
 class CrossBlock:
-    """One nonzero block ``k(f_p, u_q)`` of a multi-output sparse problem, for :func:`sparse_elbo_bwd_multi`: its flat kernel,
-    the pre-stretched points ``xg [G, 1, n_p, d]`` of ``f_p`` and ``zg [G, 1, m_q, d]`` of ``u_q``, the first column ``col`` of
+    """One nonzero block ``k(f_p, u_q)`` of a sparse problem, for :func:`sparse_elbo_bwd`: its flat kernel, the
+    pre-stretched points ``xg [G, 1, n_p, d]`` of ``f_p`` and ``zg [G, 1, m_q, d]`` of ``u_q``, the first column ``col`` of
     ``u_q`` in ``K_z``, and the optional outputs ``term_sum``, ``grad_xg`` (like ``xg``), ``grad_zg`` (like ``zg``) and
     ``param_sum`` the rectangular K1-backward accumulates into (None: not formed)."""
 
@@ -847,18 +782,22 @@ class CrossBlock:
         self.term_sum, self.grad_xg, self.grad_zg, self.param_sum = term_sum, grad_xg, grad_zg, param_sum
 
 
-def sparse_elbo_bwd_multi(procs, ch_z, ch_A, s, kdiag, kn, ybar, method, chunk, want_H=True, want_cross=True):
-    """:func:`sparse_elbo_bwd` for inducing points and observations that span several processes.  ``procs``: one entry per
-    observed process ``f_p``, in data order, ``(n_p, [CrossBlock, ...])`` (the nonzero blocks ``k(f_p, u_q)``); ``kdiag``
-    (None for DTC), ``kn`` and ``ybar``: ``[n]`` over all processes.
+def sparse_elbo_bwd(procs, ch_z, ch_A, s, kdiag, kn, ybar, method, chunk, want_H=True, want_cross=True):
+    """Backward of the sparse ELBO over chunks of data points.  ``procs``: one entry per observed process ``f_p``, in data
+    order, ``(n_p, [CrossBlock, ...])`` (the nonzero blocks ``k(f_p, u_q)``; one process with one block for a problem over
+    one inducing and one observed process); ``ch_z``: factor of ``K_z``; ``ch_A``: factor of ``A = I + W K_n^-1 W^T``;
+    ``s = A^-1 prod [m]``; ``kdiag`` (None for DTC), ``kn`` and ``ybar``: ``[n]`` over all processes.
 
     The data are walked in chunks of at most ``chunk`` points that never straddle two processes.  A chunk's rows
     ``k(x_c, z)`` are one ``c_pad x m_pad`` buffer: one K1 launch per block writes exactly ``c x m_q`` entries at the block's
     column offset (no padding flag: a padded launch would write past ``m_q`` into the next block), and the columns of zero
-    blocks and the ragged rows are zeroed.  The stages after it are those of :func:`sparse_elbo_bwd`; with ``want_cross``
-    the rectangular K1-backward then runs once per block on its column slice of the rows ``dE/dk(x_i, z)``.  Returns
-    ``(g_kn [n], g_kd [n] or None, g_ybar [n], H [1, m_pad, m_pad] or None)``.  Device memory: four ``chunk x m_pad``
-    buffers and three ``m_pad x m_pad`` ones."""
+    blocks and the ragged rows are zeroed.  The solve against ``L_z`` gives ``W_c`` (the forward's launches),
+    ``U_c = W_c A^-1``, and ``gpk_sparse_rows_bwd`` turns ``U_c`` into ``G_c`` (rows ``dE/dw_i``) and writes the per-point
+    gradients.  With ``want_H``, ``H += G_c^T W_c`` on the lower tiles (mirrored after the last chunk;
+    ``dE/dK_z = -1/2 L^-T H L^-1``).  With ``want_cross``, the transposed solve turns ``G_c`` into rows ``dE/dk(x_i, z)`` and
+    the rectangular K1-backward runs once per block on its column slice, accumulating into the block's outputs.  Returns
+    ``(g_kn [n], g_kd [n] or None, g_ybar [n], H [1, m_pad, m_pad] or None)``.  Device memory: four ``chunk x m_pad`` buffers
+    and three ``m_pad x m_pad`` ones."""
     _require_cuda(kdiag, kn, ybar)
     meth = SPARSE_METHOD[method]
     m, m_pad, dt, dev = ch_z.n, ch_z.n_pad, ch_z.dtype, ch_z.device

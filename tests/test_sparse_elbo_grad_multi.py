@@ -1,7 +1,7 @@
 """Analytic gradient of the sparse ELBO when the inducing points and / or the observations span several processes
-(``PseudoObs*((u1(z1), u2(z2)), (f1(x1, n1), y1), ...)`` under grad; ``autograd.multi_sparse_elbo``,
-``ops.sparse_elbo_bwd_multi``) against torch fp64 autograd through the same ELBO written from blocks assembled with
-``generic_grad.kernel_torch``, in the formula of ``generic_grad.sparse_compute_torch``.
+(``PseudoObs*((u1(z1), u2(z2)), (f1(x1, n1), y1), ...)`` under grad; ``autograd.sparse_elbo``, ``ops.sparse_elbo_bwd``, the
+route of single-process problems too, with one block per process pair) against torch fp64 autograd through the same ELBO
+written from blocks assembled with ``generic_grad.kernel_torch``, in the formula of ``generic_grad.sparse_compute_torch``.
 
 Three models cover the three multi-output forms: ``mix4`` (inducing points on two independent latents, observations of a
 mixture ``f1 + 2 f2`` and of ``f1``: zero blocks and sums of scaled kernels), ``shared2`` (one set of inducing points serving two

@@ -766,22 +766,27 @@ def _map_kernel(k, kind, params):
     return MappedKernel(k, m1, m2)
 
 
-def flat_under_maps(k, x, y=None):
-    """``k(x, y)`` as one flat kernel at mapped points, for the analytic gradient routes: ``(flat, scales, xm, ym)`` with
-    ``flat, scales`` the :meth:`Kernel._flat` of the kernel inside a chain of :class:`MappedKernel` s (``shift``, ``stretch``,
-    ``select``, ``periodic``, ``transform``, nested in any order; no chain: ``k`` itself) and ``xm``, ``ym`` the
-    :class:`Input` s the chain makes of ``x`` and ``y``, with their torch graph to the raw points and to the maps' parameters.
-    ``y=None``: the square ``k(x, x)``, whose two maps must be equal at every link (then ``ym is xm``); else each argument
-    takes its own maps.  None when the kernel inside does not flatten to one descriptor with terms (sums or products of
-    differently mapped kernels, derivatives, ...)."""
+def k1_block(k, x, y=None, *, through_maps=False, zero=False):
+    """``k(x, y)`` as one K1 descriptor: ``(flat, scales, xm, ym)`` with ``flat, scales`` the :meth:`Kernel._flat` of the
+    kernel and ``xm``, ``ym`` the :class:`Input` s it reads (not yet stretched by ``scales``: :meth:`Input.scaled`).  ``y=None``:
+    the square ``k(x, x)`` (then ``ym is xm``).  None for multi-output inputs, for a kernel that does not flatten to one
+    descriptor (sums or products of differently mapped kernels, derivatives, ...) and, unless ``zero``, for one without
+    terms (a zero block).
+
+    ``through_maps``: a chain of :class:`MappedKernel` s (``shift``, ``stretch``, ``select``, ``periodic``, ``transform``,
+    nested in any order) around a flat kernel resolves to that kernel at the points the chain makes of ``x`` and ``y``, with
+    their torch graph to the raw points and to the maps' parameters: only the analytic gradient routes differentiate through
+    the maps.  A square block needs equal maps at every link; a cross block maps each argument by its own."""
+    if _is_multi(x) or (y is not None and _is_multi(y)):
+        return None
     maps = []
-    while isinstance(k, MappedKernel):
+    while through_maps and isinstance(k, MappedKernel):
         if y is None and not _same_map(k.m1, k.m2):
             return None
         maps.append((k.m1, k.m2))
         k = k.k
     flat, scales = k._flat()
-    if flat is None or not flat.terms:
+    if flat is None or not (flat.terms or zero):
         return None
     xm = as_input(x)
     ym = xm if y is None else as_input(y)
@@ -1003,11 +1008,10 @@ def elwise(k, x, y=None):
 # ------------------------------------------------------------------------------------------------------------
 def _cross_rows(k_zi, z, x, ch):
     """``k_zi(z, x)^T`` as a zero-padded ``[B, m_pad, n_pad]`` row buffer (rows = points of ``x``)."""
-    if not _is_multi(x) and not _is_multi(z) and k_zi.symmetric:
-        flat, scales = k_zi._flat()
-        if flat is not None and flat.terms:
-            xi, zi = as_input(x), as_input(z)
-            return ops.kernel_rows_padded(flat, xi.scaled(scales), zi.scaled(scales), ch), xi.n
+    blk = k1_block(k_zi, z, x)
+    if blk is not None:
+        flat, scales, zi, xi = blk
+        return ops.kernel_rows_padded(flat, xi.scaled(scales), zi.scaled(scales), ch), xi.n
     Kzx = M.dense(pairwise(k_zi, z, x))  # [..., n, m]
     K3, _ = batch_flatten(Kzx, 2)
     buf = ch.new_rows(K3.shape[2])
@@ -1050,42 +1054,59 @@ def _grad_tensors(*objs):
     return out
 
 
-def _exact_route(K_z, k_zi, z, x, *others):
-    """How a posterior prediction at ``x`` is evaluated: None when no gradient is requested (the raw-pointer path), else
-    ``(args, tensors)`` -- ``args`` the inputs of :func:`autograd.exact_posterior` when the posterior is covered (exact
-    observations with a symbolic ``K_z``, a cross kernel that is one flat descriptor under input maps
-    (:func:`flat_under_maps`), single-output inputs of the factor's batch), None when it is not."""
-    multi = _is_multi(x) or _is_multi(z)
-    ts = _grad_tensors(K_z, k_zi, z, x, *others) + ([] if multi else map_output_grads(k_zi, z, x))
-    if not ts:
+def _prediction_grads(post, x, *others):
+    """The tensors that require grad behind a prediction of the exact posterior ``post`` (a :class:`PosteriorKernel` or
+    :class:`PosteriorMean`) at ``x``; ``others``: what else the prediction reads.  Empty when grad mode is off."""
+    maps = [] if _is_multi(x) or _is_multi(post.z) else map_output_grads(post.k_zi, post.z, x)
+    return _grad_tensors(post.K_z, post.k_zi, post.z, x, *others) + maps
+
+
+def _exact_args(post, x):
+    """``(flat, coefs_x, xg_x, ns, nv, coefs_c, xsg, zg, params_x, params_c)``: the cross kernel's descriptor and the tensor
+    inputs of :func:`autograd.exact_posterior` for a prediction of ``post`` at ``x``, or None when it has no analytic route.
+    Covered: exact observations with a symbolic ``K_z``, a cross kernel that is one K1 descriptor under input maps, and
+    single-output inputs of the factor's batch."""
+    K_z = post.K_z
+    blk = k1_block(post.k_zi, post.z, x, through_maps=True) if isinstance(K_z, M.KernelDense) else None
+    if blk is None:
         return None
-    res = None if multi or not isinstance(K_z, M.KernelDense) else flat_under_maps(k_zi, z, x)
-    if res is None:
-        return None, ts
-    flat, scales, zi, xi = res
+    flat, scales, zi, xi = blk
     xsg, zg = xi.scaled(scales), zi.scaled(scales)
     if xsg.shape[1] != K_z.xg.shape[1] or zg.shape[1] != K_z.xg.shape[1] or zg.shape[2] != K_z.n:
-        return None, ts
+        return None
     from .autograd import coef_tensor, param_tensor
 
     coefs_x, ns = K_z.grad_params()
-    return (flat, [coefs_x, K_z.xg, ns, K_z.noise_vec, coef_tensor(flat, xsg), xsg, zg, param_tensor(K_z.flat, K_z.xg),
-                   param_tensor(flat, xsg)]), ts
+    return (flat, coefs_x, K_z.xg, ns, K_z.noise_vec, coef_tensor(flat, xsg), xsg, zg, param_tensor(K_z.flat, K_z.xg),
+            param_tensor(flat, xsg))
 
 
-def _exact_posterior(K_z, route, ybar, fwd, half_y=None, P=None):
-    """``(dot, sq, cov)`` from ``fwd()`` with the analytic backward of ``autograd.exact_posterior``."""
-    from .autograd import PosteriorSpec, exact_posterior
+def _posterior_call(post, x, fwd, what, *others, mean=False, P=None, cross=None):
+    """``(dot, sq, cov)`` as ``fwd()`` computes them -- the launches of a prediction of the exact posterior ``post`` at ``x``,
+    None for outputs not formed -- on the prediction's gradient route:
 
-    flat, (coefs_x, xg_x, ns, nv, coefs_c, xsg, zg, params_x, params_c) = route
-    spec = PosteriorSpec(K_z.chol(), K_z.flat, flat, half_y, fwd)
+    * nothing requires grad (:func:`_prediction_grads`; ``others``: what else the prediction reads): ``fwd()`` as it is;
+    * the prediction is covered (:func:`_exact_args`): the analytic backward of ``autograd.exact_posterior``.  ``mean``:
+      ``post`` is a :class:`PosteriorMean` whose mean the prediction forms; ``P``: the prior covariance of ``cov``;
+    * else: each output attached by ``autograd.no_gradient`` to those tensors, named ``"{what} of a <posterior kind>"``
+      (:func:`_route_name`), or ``cross`` when it is given (a cross-covariance) and only the prediction is not covered;
+      ``what=None``: None instead, for a caller that falls back to predictions that name themselves."""
+    # y - m_z(z) itself: a mean given as a user function hides its parameters in a closure
+    ybar = post._ybar() if mean and torch.is_grad_enabled() else None
+    ts = _prediction_grads(post, x, *others, *((post.y, ybar) if mean else ()))
+    if not ts:
+        return fwd()
+    from .autograd import PosteriorSpec, exact_posterior, no_gradient
+
+    args = _exact_args(post, x)
+    if args is None and what is None:
+        return None
+    if args is None or cross is not None:
+        route = f"{what} of a {_route_name(post)}" if args is None else cross
+        return tuple(None if t is None else no_gradient(route, t, ts) for t in fwd())
+    flat, coefs_x, xg_x, ns, nv, coefs_c, xsg, zg, params_x, params_c = args
+    spec = PosteriorSpec(post.K_z.chol(), post.K_z.flat, flat, post._half_y() if mean else None, fwd)
     return exact_posterior(spec, coefs_x, xg_x, ns, nv, ybar, coefs_c, xsg, zg, P, params_x, params_c)
-
-
-def _uncovered(route, value, ts):
-    from .autograd import no_gradient
-
-    return no_gradient(route, value, ts)
 
 
 class PosteriorKernel(Kernel):
@@ -1103,57 +1124,39 @@ class PosteriorKernel(Kernel):
         return V, m
 
     def _pairwise_any(self, x, y, same):
-        org = _origin_of_input(x)
-        same_half = same and (self.k_zi is self.k_zj)
-        route = _exact_route(self.K_z, self.k_zi, self.z, x, self.k_zj, None if same else y)
-        if route is None or route[0] is None:
-            C = self._pairwise_raw(x, y, same, same_half)
-            if route is not None:
-                C = _uncovered(f"the posterior covariance of a {_route_name(self)}", C, route[1] + [C])
-            return M.Dense(C, org)
-        if not same_half:
-            C = self._pairwise_raw(x, y, same, same_half)
-            return M.Dense(_uncovered("a posterior cross-covariance between different inputs or processes", C,
-                                      route[1] + [C]), org)
-        prior = M.dense(pairwise(self.k_ij, x))
-        _, _, C = _exact_posterior(self.K_z, route[0], None, lambda: (None, None, self._cov_lower(x, prior)), P=prior)
-        return M.Dense(C, org)
+        prior = M.dense(pairwise(self.k_ij, x, None if same else y))
+        _, _, C = _posterior_call(self, x, lambda: (None, None, self._cov(x, y, same, prior)), "the posterior covariance",
+                                  self.k_zj, None if same else y, P=prior,
+                                  cross=None if self._same_half(same) else
+                                  "a posterior cross-covariance between different inputs or processes")
+        return M.Dense(C, _origin_of_input(x))
 
-    def _cov_lower(self, x, prior, V=None, m=None):
-        """``prior - V V^T`` from the lower triangle of the product, mirrored (``V``: the solved rows at ``x``).  The copy of
-        ``prior`` keeps its graph: when nothing behind ``V`` requires grad, the result's gradient is the prior's alone."""
+    def _same_half(self, same):
+        return same and self.k_zi is self.k_zj
+
+    def _cov(self, x, y, same, prior, V=None, m=None):
+        """``prior - V_x V_y^T`` (``V``: the solved rows at ``x`` when already formed); with one half for both sides, from the
+        lower triangle of the product, mirrored.  The copy of ``prior`` keeps its graph: when nothing behind ``V`` requires
+        grad, the result's gradient is the prior's alone."""
+        same_half = self._same_half(same)
         if V is None:
             V, m = self._half(self.k_zi, x)
+        Vy, my = (V, m) if same_half else self._half(self.k_zj, x if same else y)
         P3, bs = batch_flatten(prior, 2)
-        C = torch.zeros(P3.shape[0], V.shape[1], V.shape[1], dtype=P3.dtype, device=P3.device)
-        C[:, :m, :m] = P3
-        ops.gemm_nt(V, V, C, alpha=-1.0, beta=1.0, lower=True)
-        ops.symmetrize_(C, m)
-        return C[:, :m, :m].reshape(bs + (m, m))
-
-    def _pairwise_raw(self, x, y, same, same_half):
-        Vx, mx = self._half(self.k_zi, x)
-        Vy, my = (Vx, mx) if same_half else self._half(self.k_zj, x if same else y)
-        prior = M.dense(pairwise(self.k_ij, x, None if same else y))
-        P3, bs = batch_flatten(prior, 2)
-        C = torch.zeros(P3.shape[0], Vx.shape[1], Vy.shape[1], dtype=P3.dtype, device=P3.device)
-        C[:, :mx, :my] = P3
-        ops.gemm_nt(Vx, Vy, C, alpha=-1.0, beta=1.0, lower=same_half)
+        C = torch.zeros(P3.shape[0], V.shape[1], Vy.shape[1], dtype=P3.dtype, device=P3.device)
+        C[:, :m, :my] = P3
+        ops.gemm_nt(V, Vy, C, alpha=-1.0, beta=1.0, lower=same_half)
         if same_half:
-            ops.symmetrize_(C, mx)
-        return C[:, :mx, :my].reshape(bs + (mx, my))
+            ops.symmetrize_(C, m)
+        return C[:, :m, :my].reshape(bs + (m, my))
 
     def _elwise_any(self, x, y, same):
-        same_half = same and (self.k_zi is self.k_zj)
         prior = _elwise_any(self.k_ij, x, y, same)
-        route = _exact_route(self.K_z, self.k_zi, self.z, x, self.k_zj, None if same else y)
-        if route is not None and route[0] is not None and same_half:
-            _, corr, _ = _exact_posterior(self.K_z, route[0], None, lambda: (None, self._sq(x), None))
-        else:
-            corr = self._sq(x) if same_half else self._corr(x, y, same)
-            if route is not None:
-                name = "a " + _route_name(self) if route[0] is None else "a cross-covariance between different inputs"
-                corr = _uncovered(f"the posterior variance of {name}", corr, route[1])
+        same_half = self._same_half(same)
+        _, corr, _ = _posterior_call(self, x, lambda: (None, self._sq(x) if same_half else self._corr(x, y, same), None),
+                                     "the posterior variance", self.k_zj, None if same else y,
+                                     cross=None if same_half else
+                                     "the posterior variance of a cross-covariance between different inputs")
         return prior - corr.reshape(prior.shape[:-1]).unsqueeze(-1)
 
     def _sq(self, x):
@@ -1214,14 +1217,10 @@ class SubspaceKernel(Kernel):
         cross kernel flattens to one descriptor, and ``x``, ``z`` and ``A`` are single-output and unbatched; else None."""
         if _grad_tensors(self.A, self.k_zi, self.z) or not _grad_tensors(x):
             return None
-        if _is_multi(x) or _is_multi(self.z) or not self.k_zi.symmetric:
+        blk = k1_block(self.k_zi, self.z, x)
+        if blk is None or blk[2].batch_shape or blk[3].batch_shape or self.A.chol().batch != 1:
             return None
-        xi, zi = as_input(x), as_input(self.z)
-        if xi.batch_shape or zi.batch_shape or self.A.chol().batch != 1:
-            return None
-        flat, scales = self.k_zi._flat()
-        if flat is None or not flat.terms:
-            return None
+        flat, scales, zi, xi = blk
         return flat, zi.scaled(scales), xi.scaled(scales)
 
     def _elwise_any(self, x, y, same):
@@ -1233,7 +1232,11 @@ class SubspaceKernel(Kernel):
 
     def _no_grad(self, value, x, y):
         ts = _grad_tensors(self.A, self.k_zi, self.k_zj, self.z, x, y)
-        return _uncovered("a sparse (pseudo-observation) posterior", value, ts) if ts else value
+        if not ts:
+            return value
+        from .autograd import no_gradient
+
+        return no_gradient("a sparse (pseudo-observation) posterior", value, ts)
 
     def _matrix(self, x, y, same):
         return self._pairwise_any(x, y, same)
@@ -1527,20 +1530,9 @@ class PosteriorMean(Mean):
         d3, _ = batch_flatten(self.y - self.m_z.dev(self.z), 2)
         return d3[..., 0]
 
-    def _route(self, x):
-        # y - m_z(z) itself: a mean given as a user function hides its parameters in a closure
-        return _exact_route(self.K_z, self.k_zi, self.z, x, self.y, self._ybar() if torch.is_grad_enabled() else None)
-
     def dev(self, x):
         prior = self.m_i.dev(x)
-        route = self._route(x)
-        if route is None:
-            dot = self._dot(x)
-        elif route[0] is None:
-            dot = _uncovered(f"the posterior mean of a {_route_name(self)}", self._dot(x), route[1])
-        else:
-            dot, _, _ = _exact_posterior(self.K_z, route[0], self._ybar(), lambda: (self._dot(x), None, None),
-                                         half_y=self._half_y())
+        dot, _, _ = _posterior_call(self, x, lambda: (self._dot(x), None, None), "the posterior mean", mean=True)
         return prior + dot.reshape(prior.shape[:-1]).unsqueeze(-1)
 
     def render(self):
@@ -1575,34 +1567,29 @@ def _sparse_posterior(mean, kernel, x):
     """The sparse counterpart of :func:`_shared_posterior`: the ``PosteriorMean`` and ``PosteriorKernel + SubspaceKernel`` of
     one ``PseudoObs*`` problem (``AbstractPseudoObservations``) at numeric, single-output, unbatched ``x``, with one cross
     kernel that flattens to one descriptor and nothing that requires grad except ``x`` itself -- the marginals
-    :func:`_sparse_marginals` streams, differentiable in ``x``."""
+    :func:`_sparse_marginals` streams, differentiable in ``x``.  That cross kernel as :func:`k1_block` gives it, else None."""
     if not (isinstance(mean, PosteriorMean) and isinstance(kernel, SumKernel)):
-        return False
+        return None
     pk, sk, k = kernel.a, kernel.b, mean.k_zi
     if not (isinstance(pk, PosteriorKernel) and isinstance(sk, SubspaceKernel)):
-        return False
+        return None
     if not (pk.K_z is mean.K_z and pk.z is mean.z and sk.z is mean.z):
-        return False
-    if not (pk.k_zi is k and pk.k_zj is k and sk.k_zi is k and sk.k_zj is k and k.symmetric):
-        return False
-    if _is_multi(x) or _is_multi(mean.z) or as_input(x).batch_shape or as_input(mean.z).batch_shape:
-        return False
-    flat, _ = k._flat()
-    if flat is None or not flat.terms:
-        return False
-    if _grad_tensors(mean, kernel):
-        return False
-    return mean.K_z.chol().batch == 1 and sk.A.chol().batch == 1
+        return None
+    if not (pk.k_zi is k and pk.k_zj is k and sk.k_zi is k and sk.k_zj is k):
+        return None
+    blk = k1_block(k, mean.z, x)
+    if blk is None or blk[2].batch_shape or blk[3].batch_shape or _grad_tensors(mean, kernel):
+        return None
+    return blk if mean.K_z.chol().batch == 1 and sk.A.chol().batch == 1 else None
 
 
-def _sparse_marginals(mean, kernel, x, want_dot):
-    """``(mean or None, var)`` of a posterior :func:`_sparse_posterior` accepts, each ``[n, 1]``: the K1 rows at ``x`` are
-    formed once per chunk of test points and solved against ``L_z`` and against the factor of ``A`` (the mean only with
-    ``want_dot``); differentiable in ``x`` (``autograd.sparse_posterior_marginals``)."""
+def _sparse_marginals(mean, kernel, x, blk, want_dot):
+    """``(mean or None, var)`` of a posterior :func:`_sparse_posterior` accepts (``blk``: what it returned), each ``[n, 1]``:
+    the K1 rows at ``x`` are formed once per chunk of test points and solved against ``L_z`` and against the factor of ``A``
+    (the mean only with ``want_dot``); differentiable in ``x`` (``autograd.sparse_posterior_marginals``)."""
     from .autograd import SparsePosteriorSpec, sparse_posterior_marginals
 
-    xi, zi = as_input(x), as_input(mean.z)
-    flat, scales = mean.k_zi._flat()
+    flat, scales, zi, xi = blk
     spec = SparsePosteriorSpec(flat, zi.scaled(scales), mean.K_z.chol(), kernel.b.A.chol(),
                                mean._half_y()[0] if want_dot else None)
     prior_m = mean.m_i.dev(x) if want_dot else None
@@ -1613,8 +1600,9 @@ def _sparse_marginals(mean, kernel, x, want_dot):
 def marginal_var(mean, kernel, x):
     """``k.elwise(x)`` of a posterior process with mean ``mean``, ``[..., n, 1]``: the streamed sparse marginals where
     :func:`_sparse_posterior` holds, else the kernel's own element-wise evaluation."""
-    if _sparse_posterior(mean, kernel, x):
-        return _sparse_marginals(mean, kernel, x, want_dot=False)[1]
+    blk = _sparse_posterior(mean, kernel, x)
+    if blk is not None:
+        return _sparse_marginals(mean, kernel, x, blk, want_dot=False)[1]
     return _elwise_any(kernel, x, None, True)
 
 
@@ -1624,18 +1612,15 @@ def mean_var(mean, kernel, x):
     if _shared_posterior(mean, kernel) and not _is_multi(x):
         prior_m = mean.m_i.dev(x)
         prior = M.dense(pairwise(kernel.k_ij, x))
-        route = mean._route(x)
-        if route is not None and route[0] is None:
-            return mean.dev(x), pairwise(kernel, x)  # each raises on backward
 
         def fwd():
             V, m = kernel._half(kernel.k_zi, x)
-            return mean._dot(x, V, m), None, kernel._cov_lower(x, prior, V, m)
+            return mean._dot(x, V, m), None, kernel._cov(x, x, True, prior, V, m)
 
-        if route is None:
-            dot, _, C = fwd()
-        else:
-            dot, _, C = _exact_posterior(mean.K_z, route[0], mean._ybar(), fwd, half_y=mean._half_y(), P=prior)
+        out = _posterior_call(mean, x, fwd, None, mean=True, P=prior)
+        if out is None:
+            return mean.dev(x), pairwise(kernel, x)  # each raises on backward, naming itself
+        dot, _, C = out
         mu = prior_m + dot.reshape(prior_m.shape[:-1]).unsqueeze(-1)
         return mu, M.Dense(C, _origin_of_input(x))
     return mean.dev(x), pairwise(kernel, x)
@@ -1649,28 +1634,20 @@ def mean_var_diag(mean, kernel, x):
         prior_m = mean.m_i.dev(x)
         prior_v = _elwise_any(kernel.k_ij, x, None, True)
         shp = prior_m.shape[:-1]
-        flat, scales = (None, None)
-        if ch.batch == 1 and not _is_multi(kernel.z) and kernel.k_zi.symmetric:
-            flat, scales = kernel.k_zi._flat()
-        xi, zi = as_input(x), (as_input(kernel.z) if flat is not None else None)
+        blk = k1_block(kernel.k_zi, kernel.z, x) if ch.batch == 1 else None
 
         def fwd():
-            if flat is not None and flat.terms and not xi.batch_shape and not zi.batch_shape:
+            if blk is not None and not blk[2].batch_shape and not blk[3].batch_shape:
                 # K3 in ONE call: kernel rows -> tensor-core solve -> both reductions, test points streamed through a
                 # bounded buffer
+                flat, scales, zi, xi = blk
                 return ops.posterior_marginals(flat, xi.scaled(scales), zi.scaled(scales), ch, mean._half_y()[0]) + (None,)
             V, m = kernel._half(kernel.k_zi, x)
             return ops.row_dot_sq(V, m, ch.n_pad, mean._half_y()) + (None,)
 
-        route = mean._route(x)
-        if route is None:
-            dot, sq, _ = fwd()
-        elif route[0] is None:
-            dot, sq, _ = fwd()
-            dot, sq = (_uncovered(f"the posterior marginals of a {_route_name(mean)}", t, route[1]) for t in (dot, sq))
-        else:
-            dot, sq, _ = _exact_posterior(mean.K_z, route[0], mean._ybar(), fwd, half_y=mean._half_y())
+        dot, sq, _ = _posterior_call(mean, x, fwd, "the posterior marginals", mean=True)
         return prior_m + dot.reshape(shp).unsqueeze(-1), prior_v - sq.reshape(shp).unsqueeze(-1)
-    if _sparse_posterior(mean, kernel, x):
-        return _sparse_marginals(mean, kernel, x, want_dot=True)
+    blk = _sparse_posterior(mean, kernel, x)
+    if blk is not None:
+        return _sparse_marginals(mean, kernel, x, blk, want_dot=True)
     return mean.dev(x), _elwise_any(kernel, x, None, True)

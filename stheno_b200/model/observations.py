@@ -6,8 +6,8 @@ import torch
 from .. import B
 from .. import matrix as M
 from .. import ops
-from ..kernels import (PosteriorKernel, PosteriorMean, SubspaceKernel, _cross_rows, _elwise_any, _maps, num_elements,
-                       pairwise)
+from ..kernels import (PosteriorKernel, PosteriorMean, SubspaceKernel, _cross_rows, _elwise_any, _maps, k1_block,
+                       num_elements, pairwise)
 from .._util import batch_flatten, from_dev, to_dev, uprank
 from .fdd import FDD, _input_meta
 from .gp import cross
@@ -229,7 +229,7 @@ class AbstractPseudoObservations(AbstractObservations):
     def _elbo_grad(self, measure):
         """The ELBO with the analytic backward of ``autograd.sparse_elbo``, or None when the problem is not covered: every
         block ``k(u_q, u_q')``, ``k(u_q, f_p)`` (also symmetric) and, for VFE / FITC, ``k(f_p)`` has to flatten to one
-        descriptor or be zero (over one inducing and one observed process, also under input maps: :func:`_flat_block`), no
+        descriptor or be zero (over one inducing and one observed process, also under input maps: :func:`kernels.k1_block`), no
         input may have a batch dimension, the noise has to be Diagonal and the inducing noise Zero or Diagonal, and the data
         have to be on a CUDA device.  The forward runs the launches of the no-grad route."""
         from ..autograd import SparseElboSpec, coef_tensor, param_tensor, sparse_elbo
@@ -247,7 +247,7 @@ class AbstractPseudoObservations(AbstractObservations):
         spec_kz, spec_cross, spec_kx = [], [], []
         for q, (pq, zq) in enumerate(us):
             for q2, (pq2, zq2) in enumerate(us):
-                blk = _flat_block(measure.kernels[pq, pq2], zq, None if q2 == q else zq2, maps)
+                blk = k1_block(measure.kernels[pq, pq2], zq, None if q2 == q else zq2, through_maps=maps, zero=True)
                 if blk is None:
                     return None
                 flat, scales, zm, zm2 = blk
@@ -259,7 +259,7 @@ class AbstractPseudoObservations(AbstractObservations):
         for p, (pp, xp) in enumerate(fs):
             for q, (pq, zq) in enumerate(us):
                 k = measure.kernels[pq, pp]
-                blk = _flat_block(k, zq, xp, maps) if k.symmetric else None
+                blk = k1_block(k, zq, xp, through_maps=maps, zero=True) if k.symmetric else None
                 if blk is None:
                     return None
                 flat, scales, zm, xm = blk
@@ -268,7 +268,7 @@ class AbstractPseudoObservations(AbstractObservations):
                     spec_cross.append((p, q, flat))
                     cross.append((coef_tensor(flat, xg), xg, zm.scaled(scales), param_tensor(flat, xg)))
             if self.method in ("vfe", "fitc"):
-                blk = _flat_block(measure.kernels[pp], xp, None, maps)
+                blk = k1_block(measure.kernels[pp], xp, None, through_maps=maps, zero=True)
                 if blk is None:
                     return None
                 flat, scales, xm, _ = blk
@@ -402,25 +402,17 @@ class AbstractPseudoObservations(AbstractObservations):
 
     # -- the two ways to form A = I + W K_n^-1 W^T, prod = W K_n^-1 ybar and the scalars ------------------------------------
     def _stream_plan(self, measure, batch):
-        """``(flat, scales, x_input, z_input)`` when the problem can be streamed (one problem, numeric inputs, a symmetric
-        cross-kernel without input maps that fits one K1 descriptor), else None.  ``batch``: the number of problems ``K_z``
-        holds."""
-        from ..kernels import Input, _is_multi
+        """``(flat, scales, z_input, x_input)`` when the problem can be streamed (one problem, numeric unbatched inputs, a
+        cross-kernel that is one K1 descriptor: :func:`kernels.k1_block`), else None.  ``batch``: the number of problems
+        ``K_z`` holds."""
+        from ..kernels import Input
 
-        p_x, x, p_z, z = self.fdd.p, self.fdd.x, self.u.p, self.u.x
-        if batch != 1 or _is_multi(x) or _is_multi(z) or not isinstance(x, Input) or not isinstance(z, Input):
+        x, z = self.fdd.x, self.u.x
+        if batch != 1 or not isinstance(x, Input) or not isinstance(z, Input) or x.batch_shape or z.batch_shape:
             return None
-        if x.batch_shape or z.batch_shape:
-            return None
-        k_zx = measure.kernels[p_z, p_x]
-        if not k_zx.symmetric or _maps(k_zx):
-            return None
-        flat, scales = k_zx._flat()
-        if flat is None or not flat.terms:
-            return None
-        return flat, scales, x, z
+        return k1_block(measure.kernels[self.u.p, self.fdd.p], z, x)
 
-    def _accumulate_streamed(self, measure, ch_z, kn3, yb3, flat, scales, x, z):
+    def _accumulate_streamed(self, measure, ch_z, kn3, yb3, flat, scales, z, x):
         """``gpk_sparse_accumulate`` over chunks of data points: O(chunk m + m^2) device memory.  Also returns ``diag K_x``
         (None for DTC)."""
         acc = ops.SparseAccumulator(flat, z.scaled(scales), ch_z, self.method, chunk=B.sparse_chunk)
@@ -467,19 +459,6 @@ class AbstractPseudoObservations(AbstractObservations):
         det_kn = torch.log(2 * B.pi * kn3).sum(-1)
         yky = (yb3[..., 0] ** 2 / kn3).sum(-1)
         return A, prod, det_kn, yky, trace_part
-
-def _flat_block(k, a, b, maps):
-    """``k(a, b)`` (``b`` None: the square ``k(a, a)``) for the analytic ELBO as ``(flat, scales, am, bm)``: the descriptor
-    and length scales of :meth:`Kernel._flat` (no terms: a zero block) and the points it reads (``bm is am`` for the square
-    form), or None when the block has no analytic route.  A kernel with input maps is its inner descriptor at the mapped
-    points (:func:`kernels.flat_under_maps`), and only where ``maps`` allows it."""
-    from ..kernels import flat_under_maps
-
-    if _maps(k):
-        return flat_under_maps(k, a, b) if maps else None
-    flat, scales = k._flat()
-    return None if flat is None else (flat, scales, a, a if b is None else b)
-
 
 def _parts(fdd):
     """``[(process, Input), ...]`` of an FDD over one process or over a tuple of single-process FDDs, else None."""

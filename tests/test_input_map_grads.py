@@ -1,7 +1,7 @@
 """Gradients through input-mapped kernels (``periodic``, ``shift``, ``stretch``, ``select``, ``transform``) on the analytic
 routes: exact posterior predictions (``autograd.exact_posterior``) and the single-process sparse ELBO (``autograd.sparse_elbo``).
-Both see a mapped kernel as its inner flat kernel at mapped points (``kernels.flat_under_maps``); torch chains the
-gradients of the mapped points through the maps.
+Both see a mapped kernel as its inner flat kernel at mapped points (``kernels.k1_block`` with ``through_maps=True``); torch
+chains the gradients of the mapped points through the maps.
 
 The host tests check the resolver, the grad detection and the refusals on the CPU stand-in backend; the GPU tests compare
 gradients with torch fp64 autograd of dense restatements that write each map in torch."""
@@ -48,9 +48,13 @@ def _periodic(t, p):
 
 
 # ---- host: the resolver ---------------------------------------------------------------------------------------------------
-def test_resolver_each_map_kind(SB):
-    from stheno_b200.kernels import flat_under_maps
+def _resolve(k, *args):
+    from stheno_b200.kernels import k1_block
 
+    return k1_block(k, *args, through_maps=True)
+
+
+def test_k1_block_each_map_kind(SB):
     g = torch.Generator().manual_seed(1)
     x = torch.randn(9, 3, dtype=torch.float64, generator=g)
     y = torch.randn(5, 3, dtype=torch.float64, generator=g)
@@ -68,7 +72,7 @@ def test_resolver_each_map_kind(SB):
     ]
     for k, fmap in cases:
         for args in ((x,), (x, y)):
-            res = flat_under_maps(k, *args)
+            res = _resolve(k, *args)
             assert res is not None, k
             flat, scales, xm, ym = res
             want_flat, want_scales = inner._flat()
@@ -78,24 +82,24 @@ def test_resolver_each_map_kind(SB):
             assert xm.t.requires_grad == fmap(x).requires_grad  # the graph to the map's parameters
     # per-argument maps: the cross kernel resolves, the square one (two different maps at one link) does not
     k2 = inner.shift(c, None)
-    flat, _, xm, ym = flat_under_maps(k2, x, y)
+    flat, _, xm, ym = _resolve(k2, x, y)
     assert torch.equal(xm.t, x - c) and torch.equal(ym.t, y)
-    assert flat_under_maps(k2, x) is None
+    assert _resolve(k2, x) is None
     s2 = SB.EQ().stretch(2.0, 0.5)
-    _, _, xm, ym = flat_under_maps(s2, x, y)
+    _, _, xm, ym = _resolve(s2, x, y)
     assert torch.equal(xm.t, x / 2.0) and torch.equal(ym.t, y / 0.5)
 
 
-def test_resolver_plain_and_non_resolving(SB):
-    from stheno_b200.kernels import Input, flat_under_maps
+def test_k1_block_plain_and_non_resolving(SB):
+    from stheno_b200.kernels import Input
 
     x = torch.randn(6, 1, dtype=torch.float64)
     k = SB.Matern52().stretch(0.7) + 0.3 * SB.EQ()
-    flat, scales, xm, ym = flat_under_maps(k, x)
+    flat, scales, xm, ym = _resolve(k, x)
     assert isinstance(xm, Input) and xm.t is not None and ym is xm and torch.equal(xm.t, x)
     for bad in (SB.EQ().periodic(1.0) + SB.EQ(), SB.EQ().periodic(1.0) * SB.EQ().shift(0.5),
                 2.0 * SB.EQ().periodic(1.0), SB.EQ().diff(0)):
-        assert flat_under_maps(bad, x) is None and flat_under_maps(bad, x, x + 1) is None
+        assert _resolve(bad, x) is None and _resolve(bad, x, x + 1) is None
 
 
 # ---- host: grad detection -------------------------------------------------------------------------------------------------
@@ -109,7 +113,7 @@ def _exact_problem(SB, kernel, n=30, m=7):
 
 
 @pytest.mark.parametrize("which", ["period", "shift", "transform"])
-def test_grad_detection_sees_through_maps(SB, which):
+def test_prediction_grads_see_through_maps(SB, which):
     """A tensor period, a tensor shift and a transform whose output requires grad (the network's weights live in its
     closure) each make the exact posterior take the analytic route and the sparse problem want a gradient."""
     from stheno_b200 import kernels
@@ -118,10 +122,10 @@ def test_grad_detection_sees_through_maps(SB, which):
     W = _leaf([[0.7]])
     k = {"period": SB.EQ().periodic(t), "shift": SB.EQ().shift(t), "transform": SB.EQ().transform(lambda u: u @ W)}[which]
     post, xs = _exact_problem(SB, k)
-    route = post.mean._route(kernels.as_input(xs))
-    assert route is not None and route[0] is not None and route[1]
+    xi = kernels.as_input(xs)
+    assert kernels._exact_args(post.mean, xi) is not None and kernels._prediction_grads(post.mean, xi)
     with torch.no_grad():
-        assert post.mean._route(kernels.as_input(xs)) is None
+        assert not kernels._prediction_grads(post.mean, xi)
 
     f = SB.GP(k)
     z = torch.linspace(0, 4, 5, dtype=torch.float64)[:, None]
@@ -133,13 +137,13 @@ def test_grad_detection_sees_through_maps(SB, which):
     assert not obs._wants_grad(f.measure)
 
 
-def test_exact_route_refuses_sums_of_differently_mapped_kernels(SB):
+def test_exact_args_refuse_sums_of_differently_mapped_kernels(SB):
     from stheno_b200 import kernels
 
     p = _leaf(1.3)
     post, xs = _exact_problem(SB, SB.EQ().periodic(p) + SB.EQ())
-    route = post.mean._route(kernels.as_input(xs))
-    assert route[0] is None and route[1]
+    xi = kernels.as_input(xs)
+    assert kernels._exact_args(post.mean, xi) is None and kernels._prediction_grads(post.mean, xi)
     mean, var = post(xs).marginals()
     with pytest.raises(NotImplementedError):
         mean.sum().backward()

@@ -15,29 +15,13 @@ import torch
 
 from ._util import batch_flatten
 
-__all__ = ["kernel_needs_grad", "kernel_torch", "kernel_diag_torch", "sparse_compute_torch", "woodbury_terms_torch"]
+__all__ = ["kernel_torch", "kernel_diag_torch", "sparse_compute_torch", "woodbury_terms_torch"]
 
 
 def _t(v, like):
     if isinstance(v, torch.Tensor):
         return v.to(device=like.device, dtype=like.dtype)
     return torch.as_tensor(np.asarray(v, np.float64), device=like.device, dtype=like.dtype)
-
-
-def kernel_needs_grad(k):
-    """True if a coefficient, length scale or shape parameter (RQ's alpha) of the (flattenable) kernel expression ``k`` is a
-    tensor that requires grad."""
-    terms = k.flat_terms() if k is not None else None
-    if not terms:
-        return False
-    for coef, fs in terms:
-        if isinstance(coef, torch.Tensor) and coef.requires_grad:
-            return True
-        for f in fs:
-            for s in f[1:3]:
-                if isinstance(s, torch.Tensor) and s.requires_grad:
-                    return True
-    return False
 
 
 def _factor(kind, xs, ys, elwise, param=None):

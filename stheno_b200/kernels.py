@@ -269,7 +269,7 @@ class Kernel:
             return torch.zeros(x.batch_shape + (x.n, y.n), dtype=x.t.dtype, device=x.t.device)
         xg = x.scaled(scales)
         yg = xg if same else y.scaled(scales)
-        if torch.is_grad_enabled() and (_flat_needs_grad(flat) or xg.requires_grad or yg.requires_grad):
+        if _grad_tensors(flat, xg, yg):
             from .autograd import kernel_cross_grad, kernel_matrix_grad
 
             K = kernel_matrix_grad(flat, xg) if same else kernel_cross_grad(flat, xg, yg)
@@ -285,7 +285,7 @@ class Kernel:
             return torch.zeros(x.batch_shape + (x.n, 1), dtype=x.t.dtype, device=x.t.device)
         xg = x.scaled(scales)
         yg = xg if same else y.scaled(scales)
-        if torch.is_grad_enabled() and (_flat_needs_grad(flat) or xg.requires_grad or yg.requires_grad):
+        if _grad_tensors(flat, xg, yg):
             from .autograd import kernel_diag_grad, no_gradient
 
             if same:
@@ -327,11 +327,6 @@ def _value(v):
 
 def _requires_grad(v):
     return isinstance(v, torch.Tensor) and v.requires_grad
-
-
-def _flat_needs_grad(flat):
-    """True if a coefficient or shape parameter of the flat kernel was given as a tensor that requires grad."""
-    return getattr(flat, "coef_raw", None) is not None or getattr(flat, "param_raw", None) is not None
 
 
 def _as_kernel(k):
@@ -1020,8 +1015,9 @@ def _cross_rows(k_zi, z, x, ch):
 
 
 def _grad_tensors(*objs):
-    """The tensors that require grad reachable from the kernels, means, inputs, matrices and tensors ``objs`` (empty when
-    grad mode is off): what a posterior prediction depends on through raw-pointer kernels."""
+    """The tensors that require grad reachable from the kernels, K1 descriptors, means, inputs, matrices and tensors ``objs``
+    (empty when grad mode is off): what a result depends on through raw-pointer kernels.  Every choice between the raw route
+    and a differentiable one asks this."""
     from .model.fdd import FDD
 
     out, seen = [], set()
@@ -1042,8 +1038,10 @@ def _grad_tensors(*objs):
             walk(o.t)
         elif isinstance(o, FDD):
             walk(o.x)
+        elif isinstance(o, ops.FlatKernel):
+            walk([getattr(o, "coef_raw", None), getattr(o, "param_raw", None)])
         elif isinstance(o, M.KernelDense):
-            walk([getattr(o.flat, "coef_raw", None), getattr(o.flat, "param_raw", None), o.xg, o.noise_t, o.noise_vec])
+            walk([o.flat, o.xg, o.noise_t, o.noise_vec])
         elif isinstance(o, (Kernel, Mean, InputMap, M.AbstractMatrix)):
             for k, v in vars(o).items():
                 if k not in ("_chol", "_b"):

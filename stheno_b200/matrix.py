@@ -155,7 +155,7 @@ class KernelDense(Dense):
 
     ``dev`` materialises the full matrix with K1; ``chol()`` never does -- it builds the padded lower triangle
     (+ noise + jitter) in place and factorises it.  ``noise_t`` keeps a scalar noise given as a torch tensor that
-    requires grad (``needs_grad`` then routes ``logpdf`` through ``autograd.kernel_logpdf``)."""
+    requires grad (``logpdf`` then takes ``autograd.kernel_logpdf``)."""
 
     def __init__(self, flat, xg, batch_shape, noise_scalar=0.0, noise_vec=None, origin=None, noise_t=None):
         super().__init__(None, origin)
@@ -167,7 +167,9 @@ class KernelDense(Dense):
     @property
     def dev(self):
         if self._mat is None:
-            if self.needs_grad():
+            from .kernels import _grad_tensors
+
+            if _grad_tensors(self):
                 # differentiable materialisation (covariances assembled from several kernel matrices, e.g. multi-output
                 # joints): K1 forward + K1-backward through torch autograd; the diagonal noise is added with torch ops
                 from .autograd import kernel_matrix_grad
@@ -195,15 +197,6 @@ class KernelDense(Dense):
     @property
     def device(self):
         return self.xg.device
-
-    def needs_grad(self):
-        return torch.is_grad_enabled() and (
-            getattr(self.flat, "coef_raw", None) is not None
-            or getattr(self.flat, "param_raw", None) is not None
-            or self.xg.requires_grad
-            or (self.noise_t is not None and self.noise_t.requires_grad)
-            or (self.noise_vec is not None and self.noise_vec.requires_grad)
-        )
 
     def with_noise(self, scalar=0.0, vec=None, scalar_t=None):
         """``self + Diagonal`` stays symbolic."""
@@ -266,7 +259,10 @@ class BlockDense(Dense):
 
     @staticmethod
     def eligible(rows):
-        """Square grid, square diagonal blocks, every block a device matrix of one dtype, nothing that needs a graph."""
+        """Square grid, square diagonal blocks, every block a device matrix of one dtype, no kernel or dense block that needs a
+        graph."""
+        from .kernels import _grad_tensors
+
         if not rows or any(len(r) != len(rows) for r in rows):
             return False
         sizes = [b.shape[-1] for b in rows[0]]
@@ -274,9 +270,7 @@ class BlockDense(Dense):
             for j, b in enumerate(r):
                 if not isinstance(b, (Dense, Diagonal, Zero)) or tuple(b.shape[-2:]) != (sizes[i], sizes[j]):
                     return False
-                if isinstance(b, KernelDense) and b.needs_grad():
-                    return False
-                if isinstance(b, Dense) and not isinstance(b, KernelDense) and b.dev.requires_grad and torch.is_grad_enabled():
+                if isinstance(b, Dense) and _grad_tensors(b if isinstance(b, KernelDense) else b.dev):
                     return False
                 if tuple(b.shape[:-2]) != tuple(rows[0][0].shape[:-2]) or b.dtype != rows[0][0].dtype:
                     return False
@@ -490,12 +484,6 @@ class Woodbury(AbstractMatrix):
     def T(self):
         return self
 
-    def needs_grad(self, *others):
-        """True when a gradient has to flow through this matrix (or ``others``): ``logdet`` / ``iqf`` then take the
-        differentiable route of ``generic_grad.py`` (the raw-pointer Schur-complement GEMM would cut the graph)."""
-        ts = (self.lr.left, self.diag_m.diag) + tuple(others)
-        return torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in ts)
-
     def schur(self):
         """``(I + U^T D^-1 U)`` as a Dense (r x r) with its cached factor; the n r^2 product runs on the tensor-core
         GEMM (rows of ``U^T D^-1/2`` are K-contiguous)."""
@@ -571,6 +559,8 @@ def _origin(a, b):
 def add(a, b):
     """``B.add`` with structure: Zero is neutral, Diagonal + Diagonal stays diagonal, ``KernelDense + Diagonal``
     stays symbolic (``stheno/model/fdd.py:79``, ``stheno/model/observations.py:139,286``)."""
+    from .kernels import _grad_tensors
+
     if not isinstance(a, AbstractMatrix) and not isinstance(b, AbstractMatrix):
         return a + b
     if not isinstance(a, AbstractMatrix):
@@ -594,8 +584,7 @@ def add(a, b):
             return Woodbury(b, a, org)
         if isinstance(a, Woodbury):
             return Woodbury(add(a.diag_m, b), a.lr, org)
-        if isinstance(a, BlockDense) and a._mat is None and a._chol is None and not (
-                torch.is_grad_enabled() and b.diag.requires_grad):
+        if isinstance(a, BlockDense) and a._mat is None and a._chol is None and not _grad_tensors(b):
             return a.with_noise(b.diag)
         if isinstance(a, KernelDense) and a._mat is None and a._chol is None:
             if b.scalar is not None:

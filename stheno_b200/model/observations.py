@@ -296,30 +296,26 @@ class AbstractPseudoObservations(AbstractObservations):
         return sparse_elbo(spec, kz, nz, cross, kx, kn, ybar)
 
     # -- differentiable route (generic_grad.py): used only when something that feeds the ELBO requires grad -----------------
-    def _wants_grad(self, measure):
-        from ..generic_grad import kernel_needs_grad
-        from ..kernels import Input
+    def _grad_inputs(self, measure):
+        """The tensors that require grad behind the approximation (empty when grad mode is off): those of ``y``, the inputs,
+        the noises and the kernels, ``m(x)`` and ``m(z)`` (a mean given as a user function hides its parameters in a closure)
+        and the outputs of input transforms (:func:`kernels.map_output_grads`)."""
+        from ..kernels import _grad_tensors, map_output_grads
 
         if not torch.is_grad_enabled():
-            return False
-        p_x, p_z = self.fdd.p, self.u.p
+            return []
+        p_x, x, p_z, z = self.fdd.p, self.fdd.x, self.u.p, self.u.x
         ks = [measure.kernels[p_z], measure.kernels[p_z, p_x], measure.kernels[p_x]]
-        inputs = [self.fdd.x, self.u.x]
-        if isinstance(self.fdd.x, tuple) or isinstance(self.u.x, tuple):
-            # several processes: the joint kernels do not flatten, so look at the blocks (a mismatched part adds nothing)
+        if isinstance(x, tuple) or isinstance(z, tuple):
+            # several processes: the joint kernels reach their blocks only through the measure, so walk the blocks
             us, fs = _parts(self.u) or [], _parts(self.fdd) or []
             ks += [measure.kernels[a, b] for a, _ in us for b, _ in us + fs] + [measure.kernels[b] for b, _ in fs]
-            inputs += [v for _, v in us + fs]
-        if any(kernel_needs_grad(k) for k in ks):
-            return True
-        ts = [self.y]
-        for v in inputs:
-            if isinstance(v, Input):
-                ts.append(v.t)
-        for nz in (self.fdd.noise, self.u.noise):
-            if isinstance(nz, M.Diagonal):
-                ts.append(nz.diag)
-        return any(isinstance(t, torch.Tensor) and t.requires_grad for t in ts) or bool(self._map_grads(measure))
+        means = (measure.means[p_x].dev(x), measure.means[p_z].dev(z))
+        maps = [t for k, a, b in self._single_kernels(measure) or [] for t in map_output_grads(k, a, b)]
+        return _grad_tensors(self.y, x, z, self.fdd.noise, self.u.noise, ks, means) + maps
+
+    def _wants_grad(self, measure):
+        return bool(self._grad_inputs(measure))
 
     def _single_kernels(self, measure):
         """``[(k_z, z, z), (k_zx, z, x), (k_x, x, x)]`` of a problem over one inducing and one observed process with numeric
@@ -336,33 +332,18 @@ class AbstractPseudoObservations(AbstractObservations):
         ks = self._single_kernels(measure)
         return ks is not None and any(_maps(k) for k, _, _ in ks)
 
-    def _map_grads(self, measure):
-        """The tensors that require grad behind the input maps of a single-process problem's kernels: the maps' parameters,
-        the hyper-parameters of the kernels inside them and the outputs of transforms (:func:`kernels.map_output_grads`)."""
-        from ..kernels import _grad_tensors, map_output_grads
-
-        out = []
-        for k, a, b in self._single_kernels(measure) or []:
-            if _maps(k):
-                out += _grad_tensors(k) + map_output_grads(k, a, b)
-        return out
-
     def _compute_uncovered(self, measure):
         """A single-process problem with input-mapped kernels under grad.  The ELBO takes its analytic route when the kernels
         resolve under maps; every other result (and the ELBO when they do not) is the no-grad value, attached to the tensors it
         depends on by ``autograd.no_gradient``: a ``backward()`` through it raises instead of returning a partial gradient."""
         from ..autograd import no_gradient
-        from ..kernels import _grad_tensors
 
         key = id(measure)
         if key not in self._elbo:
             e = self._elbo_grad(measure)
             if e is not None:
                 self._elbo[key] = e
-        # y - m(x) and m(z) themselves: a mean given as a user function hides its parameters in a closure
-        means = (measure.means[self.fdd.p].dev(self.fdd.x), measure.means[self.u.p].dev(self.u.x))
-        ts = _grad_tensors(self.y, self.fdd.x, self.u.x, self.fdd.noise, self.u.noise, means,
-                           [k for k, _, _ in self._single_kernels(measure)]) + self._map_grads(measure)
+        ts = self._grad_inputs(measure)
         absent = [s for s in (self._K_z, self._mu, self._A, self._elbo) if key not in s]
         with torch.no_grad():
             self._compute(measure)

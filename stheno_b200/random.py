@@ -10,6 +10,7 @@ from . import B
 from . import matrix as M
 from . import ops
 from ._util import NUMPY, batch_flatten, from_dev, origin_of, to_dev, uprank
+from .kernels import _grad_tensors
 
 __all__ = ["Random", "RandomProcess", "RandomVector", "Normal"]
 
@@ -237,7 +238,7 @@ class Normal(RandomVector):
                 return self._logpdf_missing(xd, nan, var, out_origin)
         n = var.shape[-1]
         diff = xd if self.mean_is_zero else xd - self._mean_dev()
-        if isinstance(var, M.Woodbury) and var.needs_grad(diff):
+        if isinstance(var, M.Woodbury) and _grad_tensors(var, diff):
             from .generic_grad import woodbury_terms_torch
 
             ld, q = woodbury_terms_torch(var.lr.left, var.diag_m.diag, diff, B.epsilon)
@@ -251,10 +252,10 @@ class Normal(RandomVector):
                 var = M.Dense(var.dev, var.origin)
             d3, bs = batch_flatten(diff, 2)
             rhs_t = d3.transpose(1, 2).contiguous()  # [B, k, n]: right-hand sides as rows
-            if isinstance(var, M.KernelDense) and (var.needs_grad() or (torch.is_grad_enabled() and rhs_t.requires_grad)):
+            if isinstance(var, M.KernelDense) and _grad_tensors(var, rhs_t):
                 lp = var.logpdf_grad(rhs_t)  # analytic backward (autograd.py)
-            elif (not isinstance(var, M.KernelDense) and torch.is_grad_enabled()
-                  and (var.dev.requires_grad or rhs_t.requires_grad)):
+            elif not isinstance(var, M.KernelDense) and torch.is_grad_enabled() and _grad_tensors(var.dev, rhs_t):
+                # grad mode first: ``dev`` materialises a BlockDense grid, which the fused factorisation below never does
                 from .autograd import dense_logpdf
 
                 K3, _ = batch_flatten(var.dev, 2)
@@ -340,8 +341,6 @@ class Normal(RandomVector):
             E[:, :num, :n] = eps.transpose(1, 2)
             St = ops.gemm_nt(E, ch.L_lower_())
             s = St[:, :num, :n].transpose(1, 2).reshape(bs + (n, num))
-            from .kernels import _grad_tensors
-
             ts = _grad_tensors(var)
             if ts:  # L eps comes from the raw-pointer factorisation: a gradient through it would be silently wrong
                 from .autograd import no_gradient

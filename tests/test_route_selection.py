@@ -9,7 +9,13 @@ where ``no_gradient`` nodes are attached, that ``backward()`` raises and the exa
 The cases cover ``mean``, ``var``, ``marginals``, ``mean_var`` and ``logpdf`` of exact posteriors and ``PseudoObs*``
 posteriors and ELBOs, over plain, stretched, shifted, periodic and derivative kernels, multi-output observations and
 batched test points and cross-covariances, with nothing, a kernel variance or the test inputs requiring grad.  The host test runs the cases that
-the CPU stand-in backend covers; the GPU test runs every case."""
+the CPU stand-in backend covers; the GPU test runs every case.
+
+The ``source`` cases pin which route ``Normal.logpdf`` (on a kernel matrix, an assembled multi-output joint, a Woodbury and a
+diagonal covariance; ``BlockDense.eligible`` decides whether the joint stays a grid) and ``PseudoObs`` (``elbo``, ``mu``,
+``A``; streamed and, for a batched problem, materialised) take for each tensor that can require grad: a kernel variance,
+a length scale, RQ's alpha, a shift, a transform's output, the scalar and the vector noise, ``y``, the inputs, a mean
+parameter, a variance inside ``f * k`` -- or nothing, with and without grad mode."""
 import collections
 import sys
 
@@ -21,6 +27,10 @@ GRADS = ("off", "theta", "xs")
 
 _OPS = ("kernel_rows_padded", "posterior_marginals", "SparseAccumulator")
 _AUTOGRAD = ("exact_posterior", "no_gradient", "subspace_cov", "sparse_posterior_marginals", "sparse_elbo")
+# also recorded in the source cases: the raw factorisations, the differentiable log-pdfs and kernel matrices, the restatements
+_SOURCE_OPS = ("chol_from_kernel", "chol_from_dense", "_potrf")
+_SOURCE_AUTOGRAD = ("kernel_logpdf", "dense_logpdf", "kernel_matrix_grad", "kernel_cross_grad")
+_SOURCE_GENERIC = ("sparse_compute_torch", "woodbury_terms_torch")
 
 
 def _kernel(S, name, v):
@@ -108,9 +118,58 @@ def _run_cross(S, dev, call, grad):
     return [S.B.dense(k(xs, xs2)) if call == "pairwise" else k.elwise(xs, xs2)]
 
 
+SOURCES = ("off", "none", "variance", "scale", "alpha", "shift", "transform", "noise", "noise_vec", "y", "x", "mean", "fk")
+SOURCE_CALLS = ("logpdf-kernel", "logpdf-block", "logpdf-woodbury", "logpdf-diagonal", "elbo-streamed", "mu-streamed",
+                "A-streamed", "elbo-materialised", "mu-materialised", "A-materialised")
+
+
+def _run_source(S, dev, call, source):
+    """The outputs of ``call`` (``<what>-<covariance or layout>``) with the tensor named by ``source`` requiring grad."""
+    what, layout = call.split("-")
+    g = torch.Generator().manual_seed(5)
+    bs = (3,) if layout == "materialised" else ()
+    x = (torch.rand(bs + (30, 1), dtype=torch.float64, generator=g) * 4).to(dev)
+    z = torch.linspace(0, 4, 8, dtype=torch.float64).repeat(bs + (1,)).unsqueeze(-1).to(dev)
+    y = torch.sin(3 * x)
+
+    def leaf(v, *names):
+        return torch.as_tensor(v, dtype=torch.float64).to(dev).requires_grad_(source in names)
+
+    v, ell, alpha, c, m = leaf(1.3, "variance", "fk"), leaf(0.8, "scale"), leaf(1.5, "alpha"), leaf(0.3, "shift"), leaf(0.4, "mean")
+    W = leaf([[0.9]], "transform")
+    noise = leaf(torch.full(x.shape[:-1], 0.1), "noise_vec") if source == "noise_vec" else leaf(0.1, "noise")
+    x.requires_grad_(source == "x")
+    y.requires_grad_(source == "y")
+    k = {"woodbury": lambda: v * S.Linear(), "diagonal": lambda: v * S.Delta()}.get(layout, lambda: v * S.RQ(alpha).stretch(ell))()
+    if source == "shift":
+        k = k.shift(c)
+    elif source == "transform":
+        k = k.transform(lambda t: t @ W)
+    elif source == "fk":
+        k = (lambda t: 1 + 0.1 * t) * k
+    f = S.GP(m * S.OneMean(), k)
+    if what == "logpdf":
+        if layout == "block":
+            fdd, yy = S.combine((f(x, noise), y), ((2.0 * f)(x + 0.5, noise), y))
+            return [fdd.logpdf(yy)]
+        return [f(x, noise).logpdf(y)]
+    obs = S.PseudoObs(f(z), f(x, noise), y)
+    out = {"elbo": obs.elbo, "mu": obs.mu, "A": obs.A}[what](f.measure)
+    return [S.B.dense(out)]
+
+
+def _source_cases():
+    out = []
+    for call in SOURCE_CALLS:
+        skip = ("scale", "alpha", "fk") if call in ("logpdf-woodbury", "logpdf-diagonal") else ()
+        out += [("source", call, s) for s in SOURCES if s not in skip]
+    return out
+
+
 def _observe(S, dev, monkeypatch, case):
     """``(calls per entry point, sorted backward error texts)`` of one case."""
-    from stheno_b200 import autograd, kernels
+    from stheno_b200 import autograd, generic_grad, kernels
+    from stheno_b200 import matrix as M
 
     calls = collections.Counter()
 
@@ -124,14 +183,25 @@ def _observe(S, dev, monkeypatch, case):
 
         monkeypatch.setattr(owner, name, rec)
 
-    for name in _OPS:
-        wrap(kernels.ops, name)
-    for name in _AUTOGRAD:
-        wrap(autograd, name)
     kind, grad = case[0], case[-1]
+    for name in _OPS + (_SOURCE_OPS if kind == "source" else ()):
+        wrap(kernels.ops, name)
+    for name in _AUTOGRAD + (_SOURCE_AUTOGRAD if kind == "source" else ()):
+        wrap(autograd, name)
+    if kind == "source":
+        for name in _SOURCE_GENERIC:
+            wrap(generic_grad, name)
+        eligible = M.BlockDense.eligible
+
+        def rec_eligible(rows):
+            r = eligible(rows)
+            calls[f"BlockDense.eligible={r}"] += 1
+            return r
+
+        monkeypatch.setattr(M.BlockDense, "eligible", staticmethod(rec_eligible))
     run = {"plain": lambda: _run(S, dev, *case[1:]), "batched": lambda: _run(S, dev, *case[1:-1], grad, batched=True),
            "derivative": lambda: _run_derivative(S, dev, *case[1:]), "multi": lambda: _run_multi(S, dev, *case[1:]),
-           "cross": lambda: _run_cross(S, dev, *case[1:])}[kind]
+           "cross": lambda: _run_cross(S, dev, *case[1:]), "source": lambda: _run_source(S, dev, *case[1:])}[kind]
     try:
         if grad == "off":
             with torch.no_grad():
@@ -181,7 +251,7 @@ def _case_list():
     for call in ("mean", "var", "marginals", "mean_var"):
         out += [("derivative", call, g) for g in GRADS] + [("multi", call, g) for g in GRADS]
     out += [("cross", call, g) for call in ("pairwise", "elwise") for g in GRADS]
-    return out
+    return out + _source_cases()
 
 
 CASES = _case_list()
@@ -204,6 +274,8 @@ E12 = "gradients through the posterior marginals of a multi-output posterior are
 E13 = "gradients through the posterior mean of a multi-output posterior are not implemented"
 E14 = "gradients through the posterior covariance of a multi-output posterior are not implemented"
 E15 = "gradients through a sparse (pseudo-observation) approximation or posterior with input-mapped kernels are not implemented"
+E16 = ("NotImplementedError: gradients through FunctionScaledKernel inside a sparse approximation are not implemented (only sums / "
+       "products / stretches of the elementary kernels)")
 
 # case -> (calls per entry point, backward texts), on the GPU
 EXPECTED = {
@@ -477,6 +549,130 @@ EXPECTED = {
     "plain-sumprod-vfe-var-off": ({"SparseAccumulator": 1, "kernel_rows_padded": 2}, ()),
     "plain-sumprod-vfe-var-theta": ({"kernel_rows_padded": 2, "no_gradient": 2}, (E3, E7, )),
     "plain-sumprod-vfe-var-xs": ({"SparseAccumulator": 1, "exact_posterior": 1, "kernel_rows_padded": 2, "subspace_cov": 1}, ()),
+    "source-A-materialised-alpha": ({"sparse_compute_torch": 1}, ()),
+    "source-A-materialised-fk": ({"sparse_compute_torch": 1}, (E16, )),
+    "source-A-materialised-mean": ({"sparse_compute_torch": 1}, ()),
+    "source-A-materialised-noise": ({"sparse_compute_torch": 1}, ()),
+    "source-A-materialised-noise_vec": ({"sparse_compute_torch": 1}, ()),
+    "source-A-materialised-none": ({"chol_from_dense": 1, "chol_from_kernel": 1, "kernel_rows_padded": 1}, ()),
+    "source-A-materialised-off": ({"chol_from_dense": 1, "chol_from_kernel": 1, "kernel_rows_padded": 1}, ()),
+    "source-A-materialised-scale": ({"sparse_compute_torch": 1}, ()),
+    "source-A-materialised-shift": ({"chol_from_dense": 1, "chol_from_kernel": 1, "no_gradient": 4}, (E15, )),
+    "source-A-materialised-transform": ({"chol_from_dense": 1, "chol_from_kernel": 1, "no_gradient": 4}, (E15, )),
+    "source-A-materialised-variance": ({"sparse_compute_torch": 1}, ()),
+    "source-A-materialised-x": ({"sparse_compute_torch": 1}, ()),
+    "source-A-materialised-y": ({"sparse_compute_torch": 1}, ()),
+    "source-A-streamed-alpha": ({"sparse_compute_torch": 1}, ()),
+    "source-A-streamed-fk": ({"sparse_compute_torch": 1}, (E16, )),
+    "source-A-streamed-mean": ({"sparse_compute_torch": 1}, ()),
+    "source-A-streamed-noise": ({"sparse_compute_torch": 1}, ()),
+    "source-A-streamed-noise_vec": ({"sparse_compute_torch": 1}, ()),
+    "source-A-streamed-none": ({"SparseAccumulator": 1, "chol_from_dense": 1, "chol_from_kernel": 1}, ()),
+    "source-A-streamed-off": ({"SparseAccumulator": 1, "chol_from_dense": 1, "chol_from_kernel": 1}, ()),
+    "source-A-streamed-scale": ({"sparse_compute_torch": 1}, ()),
+    "source-A-streamed-shift": ({"chol_from_dense": 2, "chol_from_kernel": 2, "no_gradient": 3, "sparse_elbo": 1}, (E15, )),
+    "source-A-streamed-transform": ({"chol_from_dense": 2, "chol_from_kernel": 2, "no_gradient": 3, "sparse_elbo": 1}, (E15, )),
+    "source-A-streamed-variance": ({"sparse_compute_torch": 1}, ()),
+    "source-A-streamed-x": ({"sparse_compute_torch": 1}, ()),
+    "source-A-streamed-y": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-materialised-alpha": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-materialised-fk": ({"sparse_compute_torch": 1}, (E16, )),
+    "source-elbo-materialised-mean": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-materialised-noise": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-materialised-noise_vec": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-materialised-none": ({"chol_from_dense": 1, "chol_from_kernel": 1, "kernel_rows_padded": 1}, ()),
+    "source-elbo-materialised-off": ({"chol_from_dense": 1, "chol_from_kernel": 1, "kernel_rows_padded": 1}, ()),
+    "source-elbo-materialised-scale": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-materialised-shift": ({"chol_from_dense": 1, "chol_from_kernel": 1, "no_gradient": 4}, (E15, )),
+    "source-elbo-materialised-transform": ({"chol_from_dense": 1, "chol_from_kernel": 1, "no_gradient": 4}, (E15, )),
+    "source-elbo-materialised-variance": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-materialised-x": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-materialised-y": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-streamed-alpha": ({"SparseAccumulator": 1, "chol_from_dense": 1, "chol_from_kernel": 1, "sparse_elbo": 1}, ()),
+    "source-elbo-streamed-fk": ({"sparse_compute_torch": 1}, (E16, )),
+    "source-elbo-streamed-mean": ({"SparseAccumulator": 1, "chol_from_dense": 1, "chol_from_kernel": 1, "sparse_elbo": 1}, ()),
+    "source-elbo-streamed-noise": ({"SparseAccumulator": 1, "chol_from_dense": 1, "chol_from_kernel": 1, "sparse_elbo": 1}, ()),
+    "source-elbo-streamed-noise_vec": ({"SparseAccumulator": 1, "chol_from_dense": 1, "chol_from_kernel": 1, "sparse_elbo": 1}, ()),
+    "source-elbo-streamed-none": ({"SparseAccumulator": 1, "chol_from_dense": 1, "chol_from_kernel": 1}, ()),
+    "source-elbo-streamed-off": ({"SparseAccumulator": 1, "chol_from_dense": 1, "chol_from_kernel": 1}, ()),
+    "source-elbo-streamed-scale": ({"SparseAccumulator": 1, "chol_from_dense": 1, "chol_from_kernel": 1, "sparse_elbo": 1}, ()),
+    "source-elbo-streamed-shift": ({"chol_from_dense": 1, "chol_from_kernel": 1, "sparse_elbo": 1}, ()),
+    "source-elbo-streamed-transform": ({"chol_from_dense": 1, "chol_from_kernel": 1, "sparse_elbo": 1}, ()),
+    "source-elbo-streamed-variance": ({"SparseAccumulator": 1, "chol_from_dense": 1, "chol_from_kernel": 1, "sparse_elbo": 1}, ()),
+    "source-elbo-streamed-x": ({"SparseAccumulator": 1, "chol_from_dense": 1, "chol_from_kernel": 1, "sparse_elbo": 1}, ()),
+    "source-elbo-streamed-y": ({"SparseAccumulator": 1, "chol_from_dense": 1, "chol_from_kernel": 1, "sparse_elbo": 1}, ()),
+    "source-logpdf-block-alpha": ({"BlockDense.eligible=False": 1, "chol_from_dense": 1, "dense_logpdf": 1, "kernel_cross_grad": 2, "kernel_matrix_grad": 2}, ()),
+    "source-logpdf-block-fk": ({"BlockDense.eligible=False": 1, "chol_from_dense": 1, "dense_logpdf": 1, "kernel_cross_grad": 2, "kernel_matrix_grad": 2}, ()),
+    "source-logpdf-block-mean": ({"BlockDense.eligible=True": 1, "chol_from_dense": 1, "dense_logpdf": 1}, ()),
+    "source-logpdf-block-noise": ({"BlockDense.eligible=True": 1, "chol_from_dense": 1, "dense_logpdf": 1}, ()),
+    "source-logpdf-block-noise_vec": ({"BlockDense.eligible=True": 1, "chol_from_dense": 1, "dense_logpdf": 1}, ()),
+    "source-logpdf-block-none": ({"BlockDense.eligible=True": 1, "chol_from_dense": 1}, ()),
+    "source-logpdf-block-off": ({"BlockDense.eligible=True": 1, "_potrf": 1}, ()),
+    "source-logpdf-block-scale": ({"BlockDense.eligible=False": 1, "chol_from_dense": 1, "dense_logpdf": 1, "kernel_cross_grad": 2, "kernel_matrix_grad": 2}, ()),
+    "source-logpdf-block-shift": ({"BlockDense.eligible=False": 1, "chol_from_dense": 1, "dense_logpdf": 1, "kernel_cross_grad": 2, "kernel_matrix_grad": 2}, ()),
+    "source-logpdf-block-transform": ({"BlockDense.eligible=False": 1, "chol_from_dense": 1, "dense_logpdf": 1, "kernel_cross_grad": 2, "kernel_matrix_grad": 2}, ()),
+    "source-logpdf-block-variance": ({"BlockDense.eligible=False": 1, "chol_from_dense": 1, "dense_logpdf": 1, "kernel_cross_grad": 2, "kernel_matrix_grad": 2}, ()),
+    "source-logpdf-block-x": ({"BlockDense.eligible=False": 1, "chol_from_dense": 1, "dense_logpdf": 1, "kernel_cross_grad": 2, "kernel_matrix_grad": 2}, ()),
+    "source-logpdf-block-y": ({"BlockDense.eligible=True": 1, "chol_from_dense": 1, "dense_logpdf": 1}, ()),
+    "source-logpdf-diagonal-mean": ({}, ()),
+    "source-logpdf-diagonal-noise": ({}, ()),
+    "source-logpdf-diagonal-noise_vec": ({}, ()),
+    "source-logpdf-diagonal-none": ({}, ()),
+    "source-logpdf-diagonal-off": ({}, ()),
+    "source-logpdf-diagonal-shift": ({}, ()),
+    "source-logpdf-diagonal-transform": ({}, ()),
+    "source-logpdf-diagonal-variance": ({}, ()),
+    "source-logpdf-diagonal-x": ({}, ()),
+    "source-logpdf-diagonal-y": ({}, ()),
+    "source-logpdf-kernel-alpha": ({"chol_from_kernel": 1, "kernel_logpdf": 1}, ()),
+    "source-logpdf-kernel-fk": ({"chol_from_dense": 1, "dense_logpdf": 1, "kernel_matrix_grad": 1}, ()),
+    "source-logpdf-kernel-mean": ({"chol_from_kernel": 1, "kernel_logpdf": 1}, ()),
+    "source-logpdf-kernel-noise": ({"chol_from_kernel": 1, "kernel_logpdf": 1}, ()),
+    "source-logpdf-kernel-noise_vec": ({"chol_from_kernel": 1, "kernel_logpdf": 1}, ()),
+    "source-logpdf-kernel-none": ({"chol_from_kernel": 1}, ()),
+    "source-logpdf-kernel-off": ({"chol_from_kernel": 1}, ()),
+    "source-logpdf-kernel-scale": ({"chol_from_kernel": 1, "kernel_logpdf": 1}, ()),
+    "source-logpdf-kernel-shift": ({"chol_from_kernel": 1, "kernel_logpdf": 1}, ()),
+    "source-logpdf-kernel-transform": ({"chol_from_kernel": 1, "kernel_logpdf": 1}, ()),
+    "source-logpdf-kernel-variance": ({"chol_from_kernel": 1, "kernel_logpdf": 1}, ()),
+    "source-logpdf-kernel-x": ({"chol_from_kernel": 1, "kernel_logpdf": 1}, ()),
+    "source-logpdf-kernel-y": ({"chol_from_kernel": 1, "kernel_logpdf": 1}, ()),
+    "source-logpdf-woodbury-mean": ({"woodbury_terms_torch": 1}, ()),
+    "source-logpdf-woodbury-noise": ({"woodbury_terms_torch": 1}, ()),
+    "source-logpdf-woodbury-noise_vec": ({"woodbury_terms_torch": 1}, ()),
+    "source-logpdf-woodbury-none": ({"chol_from_dense": 1}, ()),
+    "source-logpdf-woodbury-off": ({"chol_from_dense": 1}, ()),
+    "source-logpdf-woodbury-shift": ({"woodbury_terms_torch": 1}, ()),
+    "source-logpdf-woodbury-transform": ({"woodbury_terms_torch": 1}, ()),
+    "source-logpdf-woodbury-variance": ({"woodbury_terms_torch": 1}, ()),
+    "source-logpdf-woodbury-x": ({"woodbury_terms_torch": 1}, ()),
+    "source-logpdf-woodbury-y": ({"woodbury_terms_torch": 1}, ()),
+    "source-mu-materialised-alpha": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-materialised-fk": ({"sparse_compute_torch": 1}, (E16, )),
+    "source-mu-materialised-mean": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-materialised-noise": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-materialised-noise_vec": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-materialised-none": ({"chol_from_dense": 1, "chol_from_kernel": 1, "kernel_rows_padded": 1}, ()),
+    "source-mu-materialised-off": ({"chol_from_dense": 1, "chol_from_kernel": 1, "kernel_rows_padded": 1}, ()),
+    "source-mu-materialised-scale": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-materialised-shift": ({"chol_from_dense": 1, "chol_from_kernel": 1, "no_gradient": 4}, (E15, )),
+    "source-mu-materialised-transform": ({"chol_from_dense": 1, "chol_from_kernel": 1, "no_gradient": 4}, (E15, )),
+    "source-mu-materialised-variance": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-materialised-x": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-materialised-y": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-streamed-alpha": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-streamed-fk": ({"sparse_compute_torch": 1}, (E16, )),
+    "source-mu-streamed-mean": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-streamed-noise": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-streamed-noise_vec": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-streamed-none": ({"SparseAccumulator": 1, "chol_from_dense": 1, "chol_from_kernel": 1}, ()),
+    "source-mu-streamed-off": ({"SparseAccumulator": 1, "chol_from_dense": 1, "chol_from_kernel": 1}, ()),
+    "source-mu-streamed-scale": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-streamed-shift": ({"chol_from_dense": 2, "chol_from_kernel": 2, "no_gradient": 3, "sparse_elbo": 1}, (E15, )),
+    "source-mu-streamed-transform": ({"chol_from_dense": 2, "chol_from_kernel": 2, "no_gradient": 3, "sparse_elbo": 1}, (E15, )),
+    "source-mu-streamed-variance": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-streamed-x": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-streamed-y": ({"sparse_compute_torch": 1}, ()),
 }
 
 # where the stand-in backend takes another route: the analytic sparse ELBO needs CUDA tensors, so on the host the ELBO
@@ -510,6 +706,20 @@ EXPECTED_HOST = {
     "plain-sumprod-dtc-elbo-theta": ({}, ()),
     "plain-sumprod-fitc-elbo-theta": ({}, ()),
     "plain-sumprod-vfe-elbo-theta": ({}, ()),
+    "source-A-streamed-shift": ({"chol_from_dense": 1, "chol_from_kernel": 1, "no_gradient": 4}, (E15, )),
+    "source-A-streamed-transform": ({"chol_from_dense": 1, "chol_from_kernel": 1, "no_gradient": 4}, (E15, )),
+    "source-elbo-streamed-alpha": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-streamed-mean": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-streamed-noise": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-streamed-noise_vec": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-streamed-scale": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-streamed-shift": ({"chol_from_dense": 1, "chol_from_kernel": 1, "no_gradient": 4}, (E15, )),
+    "source-elbo-streamed-transform": ({"chol_from_dense": 1, "chol_from_kernel": 1, "no_gradient": 4}, (E15, )),
+    "source-elbo-streamed-variance": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-streamed-x": ({"sparse_compute_torch": 1}, ()),
+    "source-elbo-streamed-y": ({"sparse_compute_torch": 1}, ()),
+    "source-mu-streamed-shift": ({"chol_from_dense": 1, "chol_from_kernel": 1, "no_gradient": 4}, (E15, )),
+    "source-mu-streamed-transform": ({"chol_from_dense": 1, "chol_from_kernel": 1, "no_gradient": 4}, (E15, )),
 }
 
 # cases whose routes reach GPU-only code (the streamed sparse marginals, the analytic backwards)

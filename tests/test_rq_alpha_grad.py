@@ -131,20 +131,19 @@ def test_rq_construction():
     assert str(S.RQ(np.float64(0.7))) == "RQ(0.7)"
 
 
-def test_deciders_see_alpha():
+def test_grad_tensors_see_alpha():
     import stheno_b200 as S
-    from stheno_b200 import generic_grad
-    from stheno_b200.kernels import _flat_needs_grad, _grad_tensors
+    from stheno_b200.kernels import _grad_tensors
 
     a = torch.tensor(0.7, dtype=torch.float64, requires_grad=True)
     k = 1.3 * S.RQ(a).stretch(0.8) + S.EQ()
-    assert generic_grad.kernel_needs_grad(k)
-    assert not generic_grad.kernel_needs_grad(1.3 * S.RQ(0.7).stretch(0.8) + S.EQ())
-    assert not generic_grad.kernel_needs_grad(S.RQ(torch.tensor(0.7)))  # a tensor that does not require grad
+    assert _grad_tensors(k)
+    assert not _grad_tensors(1.3 * S.RQ(0.7).stretch(0.8) + S.EQ())
+    assert not _grad_tensors(S.RQ(torch.tensor(0.7)))  # a tensor that does not require grad
     with warnings.catch_warnings():
         warnings.simplefilter("error")  # building the descriptor converts a detached alpha: no UserWarning
         flat, _ = k._flat()
-    assert flat.coef_raw is None and flat.param_raw is not None and _flat_needs_grad(flat)
+    assert flat.coef_raw is None and flat.param_raw is not None and _grad_tensors(flat)
     assert [p for p in flat.param_raw if p is not None] == [a]
     assert flat.terms[0][1][0] == ("rq", 0, 0.7)
     plain, _ = (1.3 * S.RQ(0.7).stretch(0.8) + S.EQ())._flat()

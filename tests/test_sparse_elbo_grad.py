@@ -358,6 +358,28 @@ def test_batched_problem_keeps_the_generic_route(S):
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("batched", [False, True])
+@pytest.mark.parametrize("method", METHODS)
+def test_mean_parameter_alone(S, method, batched):
+    """Only a constant mean's parameter requires grad: the ELBO takes a gradient route (the analytic one unbatched, the torch
+    restatement batched) and its gradient is the whole of ``dE/dc``, not just the part that ``y - m(x)`` carries."""
+    g = torch.Generator().manual_seed(12)
+    bs = (3,) if batched else ()
+    x, z, y = (torch.randn(bs + s, dtype=torch.float64, generator=g).cuda() for s in ((80, 2), (9, 2), (80, 1)))
+    c = torch.tensor(0.7, dtype=torch.float64, device="cuda", requires_grad=True)
+    k = 1.1 * S.EQ().stretch(1.3)
+    cls = {"vfe": S.PseudoObs, "fitc": S.PseudoObsFITC, "dtc": S.PseudoObsDTC}[method]
+    f = S.GP(c * S.OneMean(), k)
+    e = cls(f(z), f(x, 0.2), y).elbo(f.measure)
+    ones = torch.ones(bs + (9, 1), dtype=torch.float64, device="cuda")
+    want = sparse_compute_torch(method, k, k, k, z, x, torch.full(bs + (80,), 0.2, dtype=torch.float64, device="cuda"), None,
+                                y - c, c * ones, S.B.epsilon)[3]
+    (ge,) = torch.autograd.grad(e.sum(), [c])
+    (gw,) = torch.autograd.grad(want.sum(), [c])
+    assert _errors([ge], [gw])[0] <= 1e-8, (float(ge), float(gw))
+
+
+@pytest.mark.gpu
 def test_elbo_is_not_replaced_by_a_later_prediction(S):
     """The ELBO returned under grad stays the stored one when ``mu`` is asked for later (which takes the generic route)."""
     rng = np.random.default_rng(6)

@@ -17,7 +17,8 @@
  *   - Return value: 0 = launched OK; < 0 = bad argument (GPK_ERR_*) or a CUDA launch error (-1000 - cudaError).
  *     Numerical failure (non-positive pivot) is reported LAPACK-style through the device-side `info` word
  *     (index of the first bad pivot, 1-based; 0 = success) so that no host sync is forced.
- *   - `_f64` / `_f32` suffix = arithmetic type (double / float); everything is computed in that type.
+ *   - `_f64` / `_f32` suffix = arithmetic type (double / float); everything is computed in that type, except the row
+ *     reductions that say "fp64 sums in both precisions".
  *   - The one environment variable the library reads is GPK_NO_LOOKAHEAD, at every gpk_potrf_* call.  When it is set,
  *     the factorisation enqueues all its work on `stream` instead of factorising the next panel on side streams while
  *     the trailing update runs, so that CUDA events around a launch time that kernel alone.  It is meant for profiling:
@@ -175,6 +176,16 @@ int gpk_gemm_nt_f64(int64_t M, int64_t N, int64_t K, double alpha, const double*
 int gpk_gemm_nt_f32(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t lda, int64_t a_bstride,
                     const float* B, int64_t ldb, int64_t b_bstride, float beta, float* C, int64_t ldc,
                     int64_t c_bstride, int32_t lower, int32_t batch, void* stream);
+/* gpk_gemm_nt_f32 runs on the wgmma tensor cores with the 3xTF32 split (a = hi + lo, hi = a & 0xFFFFE000; a b formed as
+ * hi hi + hi lo + lo hi) when K >= 128, K % 32 == 0, every ld and batch stride is a multiple of 4 and the pointers are 16-byte
+ * aligned, and on an fp32 FFMA kernel otherwise.  Where the two differ (measured on an H100 80GB HBM3 at a 700 W power limit):
+ *   - error: FFMA is fp32 arithmetic.  3xTF32 on random normal operands gives max |err| / max(|A| |B|^T) = 3.1e-6 at K = 4096,
+ *     4.3e-6 at 8192 and 6.1e-6 at 16384 (about 0.8 u sqrt(K), u = 2^-24); the worst case is (6 K + 48) u |alpha| |A| |B|^T.
+ *   - subnormals: both keep subnormal operands and subnormal products (no flush to zero).
+ *   - non-finite inputs: on 3xTF32 a row of A (B) holding a NaN or an infinity makes its whole row (column) of alpha A B^T NaN,
+ *     where FFMA gives NaN or +-inf as fp32 does: the low part of +-inf is inf - inf = NaN.  (A low part of 0 would not give
+ *     fp32's answer either: hi lo would be inf * 0 = NaN wherever the other operand is exact in TF32.)  The opt-in
+ *     gpk_potrf_f64_tf32x3 below forms its trailing updates the same way. */
 
 /* K2: blocked right-looking Cholesky, in place, lower, row-major.
  *   A: [(n_pad + extra_rows) x n_pad] (ld = lda): the first n_pad rows hold the (padded) SPD matrix; the
@@ -222,14 +233,14 @@ int gpk_trsm_right_t_f32(const float* L, int64_t ldl, int64_t l_bstride, int64_t
                          int64_t b_bstride, int64_t rows, int32_t batch, void* stream);
 
 /* K4: log-marginal finish: out[b][c] = -0.5 * (logdet[b] + n * log(2 pi) + sum_j a[b][c][j]^2), c < k, where row c
- * of `a` (ld = lda) is (L^-1 (y_c - mu))^T.  stheno/random.py:272-279. */
+ * of `a` (ld = lda) is (L^-1 (y_c - mu))^T.  fp64 sums in both precisions, rounded once.  stheno/random.py:272-279. */
 int gpk_logpdf_finish_f64(const double* a, int64_t lda, int64_t a_bstride, int64_t n, int64_t n_cols, int32_t k,
                           const double* logdet, double* out, int32_t batch, void* stream);
 int gpk_logpdf_finish_f32(const float* a, int64_t lda, int64_t a_bstride, int64_t n, int64_t n_cols, int32_t k,
                           const float* logdet, float* out, int32_t batch, void* stream);
 
 /* Row reductions over V (rows x n_cols, ld = ldv):  dot[r] = sum_j V[r][j] * b[j] (b may be NULL),
- * sq[r] = sum_j V[r][j]^2 (sq may be NULL).  Posterior mean  m(x*) + V b  and marginal variance
+ * sq[r] = sum_j V[r][j]^2 (sq may be NULL); fp64 sums in both precisions, rounded once.  Posterior mean  m(x*) + V b  and marginal variance
  * k(x*,x*) - sum V^2 (mlkernels mean_var_diag via stheno/model/fdd.py:72-74); B.matmul_diag at observations.py:305. */
 int gpk_row_dot_sq_f64(const double* V, int64_t ldv, int64_t v_bstride, int64_t rows, int64_t n_cols,
                        const double* b, int64_t b_bstride, double* dot, double* sq, int64_t o_bstride,

@@ -58,6 +58,8 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, i
       : "memory");
 }
 
+// Exact for every finite value, subnormals included.  For +-inf it is inf - inf = NaN, so a row holding an infinity comes out
+// NaN (include/gpk.h, tests/test_fp32_route.py).
 __device__ __forceinline__ float4 tf32_low_part(float4 v) {
   float4 lo;
   lo.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u);

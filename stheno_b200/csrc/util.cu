@@ -9,30 +9,31 @@ namespace gpk {
 long long g_launch_count = 0;
 
 // ---- logpdf finish: out[b][c] = -0.5 (logdet[b] + n log 2pi + sum_j a[b][c][j]^2) -------------------------------
-// stheno/random.py:272-279.  One CTA per (c, b); a HBM-read-bound row reduction.
+// stheno/random.py:272-279.  One CTA per (c, b); a HBM-read-bound row reduction.  fp64 sums in both precisions: in fp32,
+// each thread adds n_cols / 512 terms in sequence, and a running sum near 1 would drop every term below 2^-25.
 template <typename T>
 __global__ void logpdf_finish_kernel(const T* __restrict__ a, int64_t lda, int64_t a_bs, int64_t n, int64_t n_cols,
                                      int32_t k, const T* __restrict__ logdet, T* __restrict__ out) {
   const int c = blockIdx.x, b = blockIdx.y;
   const T* row = a + (int64_t)b * a_bs + (int64_t)c * lda;
-  T s = T(0);
+  double s = 0.0;
   for (int64_t j = threadIdx.x; j < n_cols; j += blockDim.x) {
-    const T v = row[j];
+    const double v = (double)row[j];
     s = fma(v, v, s);
   }
-  __shared__ T red[32];
+  __shared__ double red[32];
   s = warp_sum(s);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
   __syncthreads();
   if (threadIdx.x == 0) {
-    T t = T(0);
+    double t = 0.0;
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w];
-    const T log2pi = T(1.8378770664093454835606594728112);
-    out[(int64_t)b * k + c] = -(logdet[b] + (T)n * log2pi + t) / T(2);
+    const double log2pi = 1.8378770664093454835606594728112;
+    out[(int64_t)b * k + c] = (T)(-((double)logdet[b] + (double)n * log2pi + t) / 2.0);
   }
 }
 
-// ---- row reductions: dot[r] = <V[r,:], b>, sq[r] = |V[r,:]|^2 ; one warp per row ----------------------------------
+// ---- row reductions: dot[r] = <V[r,:], b>, sq[r] = |V[r,:]|^2 ; one warp per row, fp64 sums in both precisions ---------
 template <typename T>
 __global__ void row_dot_sq_kernel(const T* __restrict__ V, int64_t ldv, int64_t v_bs, int64_t rows, int64_t n_cols,
                                   const T* __restrict__ bvec, int64_t b_bs, T* __restrict__ dot, T* __restrict__ sq,
@@ -43,17 +44,17 @@ __global__ void row_dot_sq_kernel(const T* __restrict__ V, int64_t ldv, int64_t 
   const int lane = threadIdx.x & 31;
   const T* row = V + (int64_t)bidx * v_bs + r * ldv;
   const T* bv = bvec ? bvec + (int64_t)bidx * b_bs : nullptr;
-  T sd = T(0), ss = T(0);
+  double sd = 0.0, ss = 0.0;
   for (int64_t j = lane; j < n_cols; j += 32) {
-    const T v = row[j];
+    const double v = (double)row[j];
     ss = fma(v, v, ss);
-    if (bv) sd = fma(v, bv[j], sd);
+    if (bv) sd = fma(v, (double)bv[j], sd);
   }
   sd = warp_sum(sd);
   ss = warp_sum(ss);
   if (lane == 0) {
-    if (dot) dot[(int64_t)bidx * o_bs + r] = sd;
-    if (sq) sq[(int64_t)bidx * o_bs + r] = ss;
+    if (dot) dot[(int64_t)bidx * o_bs + r] = (T)sd;
+    if (sq) sq[(int64_t)bidx * o_bs + r] = (T)ss;
   }
 }
 

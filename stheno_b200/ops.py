@@ -262,10 +262,16 @@ def row_dot_sq(V, rows, n_cols, b=None, want_dot=True, want_sq=True):
     sq = torch.empty(Bn, rows, device=V.device, dtype=V.dtype) if want_sq else None
     if rows == 0:
         return dot, sq
+    b_bs = 0
     if b is not None:
         b = b.contiguous()
+        if b.dim() > 1 and b.shape[0] != Bn:  # one vector for a batch of row sets (the test-point sets of one problem)
+            if b.shape[0] != 1:
+                raise ValueError(f"row_dot_sq: {b.shape[0]} vectors against {Bn} row sets")
+        elif b.dim() > 1:
+            b_bs = b.stride(0)
     rc = _fn("gpk_row_dot_sq", V.dtype)(
-        _ptr(V), V.stride(1), V.stride(0), rows, n_cols, _ptr(b), (b.stride(0) if b is not None else 0), _ptr(dot),
+        _ptr(V), V.stride(1), V.stride(0), rows, n_cols, _ptr(b), b_bs, _ptr(dot),
         _ptr(sq), rows, Bn, _stream(),
     )
     check(rc, "gpk_row_dot_sq")
@@ -344,10 +350,11 @@ class Chol:
         if Bt.shape[2] != self.n_pad or Bt.shape[1] % TILE or Bt.stride(2) != 1:
             raise ValueError("solve_rows_ needs a padded [B, rows_pad, n_pad] buffer")
         Lp = self.L_padded()
-        rows, n_pad, batch = Bt.shape[1], self.n_pad, self.batch
+        rows, n_pad, batch = Bt.shape[1], self.n_pad, Bt.shape[0]
         em = _emulation(self.dtype, self.device, lambda lib, s: lib.gpk_trsm_right_oz_ws_bytes(n_pad, rows, s) if batch == 1 else 0)
         rc = _fn("gpk_trsm_right", self.dtype)(
-            _ptr(Lp), Lp.stride(1), Lp.stride(0), n_pad, _ptr(Bt), Bt.stride(1), Bt.stride(0), rows, batch, *em, _stream(),
+            _ptr(Lp), Lp.stride(1), self._batch_stride(Bt), n_pad, _ptr(Bt), Bt.stride(1), Bt.stride(0), rows, batch, *em,
+            _stream(),
         )
         check(rc, "gpk_trsm_right")
         return Bt
@@ -357,11 +364,20 @@ class Chol:
         _require_cuda(Bt)
         Lp = self.L_padded()
         rc = _fn("gpk_trsm_right_t", self.dtype)(
-            _ptr(Lp), Lp.stride(1), Lp.stride(0), self.n_pad, _ptr(Bt), Bt.stride(1), Bt.stride(0), Bt.shape[1],
-            self.batch, _stream(),
+            _ptr(Lp), Lp.stride(1), self._batch_stride(Bt), self.n_pad, _ptr(Bt), Bt.stride(1), Bt.stride(0), Bt.shape[1],
+            Bt.shape[0], _stream(),
         )
         check(rc, "gpk_trsm_right_t")
         return Bt
+
+    def _batch_stride(self, Bt):
+        """The batch stride of ``L`` for the row buffer ``Bt``: one factor solves every member of a batch of row sets (the
+        test-point sets of one problem) through stride 0; otherwise ``Bt`` has one member per factor."""
+        if Bt.shape[0] == self.batch:
+            return self.L_padded().stride(0)
+        if self.batch != 1:
+            raise ValueError(f"row buffer batch {Bt.shape[0]} against {self.batch} factors")
+        return 0
 
     def solve_many_rows_t_(self, Bt, leaf=1024, panel=1024):
         """:meth:`solve_rows_t_` for many rows (a chunk of test points).  ``gpk_trsm_right_t`` is a CUDA-core backward
@@ -371,6 +387,8 @@ class Chol:
         _require_cuda(Bt)
         if Bt.shape[2] != self.n_pad or Bt.shape[1] % TILE or Bt.stride(2) != 1:
             raise ValueError("solve_many_rows_t_ needs a padded [B, rows_pad, n_pad] buffer")
+        if Bt.shape[0] != self.batch:
+            raise ValueError(f"solve_many_rows_t_: row buffer batch {Bt.shape[0]} against {self.batch} factors")
         self._solve_t_block(Bt, 0, self.n_pad, leaf, panel)
         return Bt
 
@@ -598,6 +616,10 @@ def kernel_rows_padded(flat, xsg, xg, chol):
     _check_groups(xg, flat)
     B, m, d = xsg.shape[1], xsg.shape[2], xsg.shape[3]
     n = xg.shape[2]
+    if xg.shape[1] != B:  # one problem, a batch of test-point sets: every set reads the same data points
+        if xg.shape[1] != 1:
+            raise ValueError(f"kernel_rows_padded: data batch {xg.shape[1]} against test-point batch {B}")
+        xg = xg.expand(-1, B, -1, -1)
     out = torch.empty(B, round_up(max(m, 1)), chol.n_pad, device=xg.device, dtype=xg.dtype)
     _km_launch(flat, xsg, xg, m, n, d, KM_PAD_ZERO, 0.0, None, 0.0, out, out.stride(1), out.stride(0), B)
     return out

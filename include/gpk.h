@@ -354,6 +354,20 @@ int gpk_sparse_rows_bwd_f32(int64_t c, int64_t m_pad, const float* Wc, int64_t l
                             const float* q, const float* kdiag, const float* kn, const float* ybar, int32_t method,
                             float* g_kn, float* g_kd, float* g_ybar, void* stream);
 
+/* Random-feature evaluation of a pathwise function sample (stheno_b200/pathwise.py):
+ *   out[i][s] = (accumulate ? out[i][s] : 0) + sum_j W[s][j] amp[j] cos(x_i . omega[j] + b[j]),   i < n, s < num
+ * x: [n x d] (ld = ldx), omega: [F x d] dense (already divided by the length scales), b, amp: [F], W: [num x F] (ld = ldw),
+ * out: [n x num] (ld = ldo).  The n x F feature matrix is never written to memory: feature blocks are formed in shared memory
+ * or registers and contracted at once, on the fp64 tensor cores (DMMA) for the fp64 entry point with num >= 8 and by
+ * CUDA-core FMAs otherwise.  The phase x . omega + b is formed in fp64 in both precisions and its cosine is the library one
+ * (full accuracy at large arguments); the fp32 entry point sums in fp32.  A row of x holding a NaN gives a NaN row. */
+int gpk_feature_eval_f64(const double* x, int64_t ldx, int64_t n, int32_t d, const double* omega, const double* b,
+                         const double* amp, int64_t F, const double* W, int64_t ldw, int32_t num, double* out, int64_t ldo,
+                         int32_t accumulate, void* stream);
+int gpk_feature_eval_f32(const float* x, int64_t ldx, int64_t n, int32_t d, const float* omega, const float* b,
+                         const float* amp, int64_t F, const float* W, int64_t ldw, int32_t num, float* out, int64_t ldo,
+                         int32_t accumulate, void* stream);
+
 /* Measurement helper (bench.py): runs a register-resident fp64 tensor-core (DMMA) loop on every SM and returns the
  * achieved TFLOP/s -- the denominator of the fp64 roofline -- or a negative error code.  Synchronises the device. */
 double gpk_probe_dmma_tflops(void);

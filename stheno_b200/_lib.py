@@ -61,6 +61,7 @@ _SIGNATURES = {
     "gpk_sparse_accumulate": [POINTER(KernelDesc), _ptr, _i64, _i64, _ptr, _i64, _i64, _i32, _ptr, _i64, _i64, _ptr, _ptr, _ptr,
                               _i32, _ptr, _i64, _ptr, _ptr, _ptr, _i64, "OZ", _ptr],
     "gpk_sparse_rows_bwd": [_i64, _i64, _ptr, _i64, _ptr, _i64, _ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _ptr],
+    "gpk_feature_eval": [_ptr, _i64, _i64, _i32, _ptr, _ptr, _ptr, _i64, _ptr, _i64, _i32, _ptr, _i64, _i32, _ptr],
 }
 _PLAIN = {
     "gpk_version": ([], c_int32),

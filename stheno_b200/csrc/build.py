@@ -8,7 +8,7 @@ import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["kernel_matrix.cu", "kernel_matrix_bwd.cu", "gemm.cu", "gemm_tc32.cu", "gemm_oz.cu", "potrf.cu", "util.cu", "sparse.cu", "posterior.cu"]
+SOURCES = ["kernel_matrix.cu", "kernel_matrix_bwd.cu", "gemm.cu", "gemm_tc32.cu", "gemm_oz.cu", "potrf.cu", "util.cu", "sparse.cu", "posterior.cu", "sample_fn.cu"]
 LIB = os.path.join(HERE, "libgpk.so")
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

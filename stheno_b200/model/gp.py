@@ -191,6 +191,16 @@ class GP(RandomProcess):
             df = df + float(c) * self.shift(float(-g * step))
         return df / step**deriv
 
+    def sample_function(self, num=1, features=4096, state=None):
+        """``num`` functions drawn from this GP -- prior or exact posterior -- as one
+        :class:`~stheno_b200.pathwise.FunctionSample`: call it at any points, any number of times, and it evaluates the same
+        functions (pathwise conditioning of a ``features``-feature random-Fourier prior sample).  ``state``: a
+        ``torch.Generator`` that makes the draw reproducible.  Refuses with ``ValueError`` what it does not cover (products of
+        kernel factors, Delta terms, derivative or function-scaled kernels, multi-output, sparse and cross-process posteriors)."""
+        from ..pathwise import FunctionSample
+
+        return FunctionSample(self, num=num, features=features, state=state)
+
     @property
     def stationary(self):
         return self.kernel.stationary

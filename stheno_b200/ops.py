@@ -222,6 +222,32 @@ def gemm_nt(A, Bm, C=None, *, alpha=1.0, beta=0.0, lower=False):
     return C
 
 
+def feature_eval(x, omega, b, amp, W, out=None, chunk=1 << 20):
+    """``out[i, s] (+)= sum_j W[s, j] amp[j] cos(x_i . omega_j + b_j)`` (``gpk_feature_eval``): ``x [n, d]``, ``omega [F, d]``,
+    ``b, amp [F]``, ``W [num, F]`` -> ``[n, num]``.  With ``out`` (a ``[n, num]`` tensor with a unit inner stride) the sum is
+    added to it, else a new tensor is returned.  Rows are launched ``chunk`` at a time; the ``n x F`` features are never held."""
+    _require_cuda(x, omega, b, amp, W, out)
+    x, omega, b, amp, W = [t.contiguous() for t in (x, omega, b, amp, W)]
+    n, d = x.shape
+    F, num = omega.shape[0], W.shape[0]
+    if omega.shape[1] != d or b.shape != (F,) or amp.shape != (F,) or W.shape[1] != F:
+        raise ValueError("feature_eval: shapes do not match")
+    if any(t.dtype != x.dtype for t in (omega, b, amp, W, out) if t is not None):
+        raise TypeError("feature_eval: x, omega, b, amp, W and out must share one dtype")
+    accumulate = out is not None
+    if out is None:
+        out = torch.empty(n, num, device=x.device, dtype=x.dtype)
+    elif out.shape != (n, num) or out.stride(1) != 1:
+        raise ValueError("feature_eval: out must be [n, num] with a unit inner stride")
+    fn = _fn("gpk_feature_eval", x.dtype)
+    for a in range(0, n, chunk):
+        c = min(n, a + chunk) - a
+        rc = fn(_ptr(x[a]), d, c, d, _ptr(omega), _ptr(b), _ptr(amp), F, _ptr(W), F, num, _ptr(out[a]), out.stride(0),
+                1 if accumulate else 0, _stream())
+        check(rc, "gpk_feature_eval")
+    return out
+
+
 def _pad_copy(src, dst, rows, cols, rows_pad, cols_pad, diag_add, pad_identity):
     if src.stride(2) != 1:
         src = src.contiguous()

@@ -54,9 +54,10 @@ def _n_factors(flat):
 
 class _KernelLogpdf(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, coefs, xg, noise_scalar, noise_vec, rhs_t, structure, jitter, params):
-        # coefs [T], xg [G, B, n, d], noise_scalar [] , noise_vec [B, n] or None, rhs_t [B, k, n]
-        flat = ops.FlatKernel([(float(c), fs) for c, fs in zip(coefs.tolist(), structure)], xg.shape[0])
+    def forward(ctx, flat, coefs, xg, noise_scalar, noise_vec, rhs_t, jitter, params):
+        # flat: the caller's descriptor, which the launches read (as in the three functions below); coefs [T] and params [F]
+        # (coef_tensor, param_tensor) only route the gradients of its hyper-parameters to those given as tensors
+        # xg [G, B, n, d], noise_scalar [] , noise_vec [B, n] or None, rhs_t [B, k, n]
         # the backward reads alpha and K^-1 element by element off this factor: never the 7-slice factorisation
         ch = ops.chol_from_kernel(flat, xg.detach().contiguous(), noise_scalar=float(noise_scalar),
                                   noise_vec=None if noise_vec is None else noise_vec.detach(), jitter=jitter,
@@ -77,7 +78,7 @@ class _KernelLogpdf(torch.autograd.Function):
         grad_noise_scalar = diag.sum()
         grad_noise_vec = diag if ctx.has_nv else None
         grad_rhs = -g.unsqueeze(-1) * alpha
-        return grad_coefs, grad_xg, grad_noise_scalar, grad_noise_vec, grad_rhs, None, None, _param_grad(flat, ps)
+        return None, grad_coefs, grad_xg, grad_noise_scalar, grad_noise_vec, grad_rhs, None, _param_grad(flat, ps)
 
 
 def _alpha_and_G(ch, g):
@@ -142,8 +143,7 @@ class _KernelMatrix(torch.autograd.Function):
     """Differentiable ``k(x, x)`` (same points) built by K1; backward = K1-backward on the symmetrised upstream gradient."""
 
     @staticmethod
-    def forward(ctx, coefs, xg, structure, params):
-        flat = ops.FlatKernel([(float(c), fs) for c, fs in zip(coefs.tolist(), structure)], xg.shape[0])
+    def forward(ctx, flat, coefs, xg, params):
         ctx.flat, ctx.xg = flat, xg.detach().contiguous()
         return ops.kernel_matrix(flat, ctx.xg)
 
@@ -154,12 +154,11 @@ class _KernelMatrix(torch.autograd.Function):
         Gs = (0.5 * (G + G.transpose(1, 2))).contiguous()  # K is symmetric: only the symmetric part of G matters
         ps = _param_buf(ctx.needs_input_grad[3], xg.shape[1], xg)
         term_sum, grad_xg, _ = _bwd_kernel(flat, xg, Gs, n, ps)
-        return term_sum[:, : len(flat.terms)].sum(0), grad_xg, None, _param_grad(flat, ps)
+        return None, term_sum[:, : len(flat.terms)].sum(0), grad_xg, _param_grad(flat, ps)
 
 
 def _scalar(v, like):
-    """``v`` as a 0-d tensor of ``like``'s dtype and device; a float is converted straight to that dtype (through torch's
-    float32 default it would lose its low bits, and the descriptor built from the tensor with them)."""
+    """``v`` as a 0-d tensor of ``like``'s dtype and device, with its graph when it is a tensor."""
     if isinstance(v, torch.Tensor):
         return v.to(device=like.device, dtype=like.dtype).reshape(())
     return torch.tensor(float(v), device=like.device, dtype=like.dtype)
@@ -183,25 +182,22 @@ def param_tensor(flat, like):
 
 def kernel_matrix_grad(flat, xg):
     """``k(x, x) [B, n, n]`` with an autograd graph to the kernel's tensor hyper-parameters and to ``xg``."""
-    return _KernelMatrix.apply(coef_tensor(flat, xg), xg, [fs for _, fs in flat.terms], param_tensor(flat, xg))
+    return _KernelMatrix.apply(flat, coef_tensor(flat, xg), xg, param_tensor(flat, xg))
 
 
-def kernel_logpdf(coefs, xg, noise_scalar, noise_vec, rhs_t, structure, jitter, params=None):
-    """Differentiable ``logpdf`` ``[B, k]`` of ``N(0, sum_t coefs[t] prod phi(xg) + noise + jitter I)`` at ``rhs_t``;
-    ``params``: the factors' shape parameters (:func:`param_tensor`), for their gradient."""
-    return _KernelLogpdf.apply(coefs, xg, noise_scalar, noise_vec, rhs_t, structure, jitter, params)
-
-
-def _flat_of(coefs, structure, n_groups):
-    return ops.FlatKernel([(float(c), fs) for c, fs in zip(coefs.tolist(), structure)], n_groups)
+def kernel_logpdf(flat, xg, noise_scalar, noise_vec, rhs_t, jitter):
+    """Differentiable ``logpdf`` ``[B, k]`` of ``N(0, k(x, x) + noise + jitter I)`` at ``rhs_t`` for the flat kernel ``flat``
+    on ``xg``, with an autograd graph to the kernel's tensor hyper-parameters, ``xg``, the noise (``noise_scalar``: a float
+    or a tensor; ``noise_vec [B, n]`` or None) and ``rhs_t``."""
+    return _KernelLogpdf.apply(flat, coef_tensor(flat, xg), xg, _scalar(noise_scalar, xg), noise_vec, rhs_t, jitter,
+                               param_tensor(flat, xg))
 
 
 class _KernelCross(torch.autograd.Function):
     """Differentiable ``k(x, y)`` for two different point sets, built by K1; backward = the rectangular K1-backward."""
 
     @staticmethod
-    def forward(ctx, coefs, xsg, xg, structure, params):
-        flat = _flat_of(coefs, structure, xsg.shape[0])
+    def forward(ctx, flat, coefs, xsg, xg, params):
         ctx.flat, ctx.xsg, ctx.xg = flat, xsg.detach().contiguous(), xg.detach().contiguous()
         return ops.kernel_matrix(flat, ctx.xsg, ctx.xg, same=False)
 
@@ -209,26 +205,25 @@ class _KernelCross(torch.autograd.Function):
     def backward(ctx, G):
         flat, xsg, xg = ctx.flat, ctx.xsg, ctx.xg
         nig = ctx.needs_input_grad
-        ts = torch.zeros(xsg.shape[1], _lib.GPK_MAX_TERMS, dtype=xsg.dtype, device=xsg.device) if nig[0] else None
-        gxs = torch.zeros_like(xsg) if nig[1] else None
-        gx = torch.zeros_like(xg) if nig[2] else None
+        ts = torch.zeros(xsg.shape[1], _lib.GPK_MAX_TERMS, dtype=xsg.dtype, device=xsg.device) if nig[1] else None
+        gxs = torch.zeros_like(xsg) if nig[2] else None
+        gx = torch.zeros_like(xg) if nig[3] else None
         ps = _param_buf(nig[4], xsg.shape[1], xsg)
         ops.kernel_cross_bwd(flat, xsg, xg, W=G.contiguous(), term_sum=ts, grad_xsg=gxs, grad_xg=gx, param_sum=ps)
-        return None if ts is None else ts[:, : len(flat.terms)].sum(0), gxs, gx, None, _param_grad(flat, ps)
+        return None, None if ts is None else ts[:, : len(flat.terms)].sum(0), gxs, gx, _param_grad(flat, ps)
 
 
 def kernel_cross_grad(flat, xsg, xg):
     """``k(x, y) [B, m, n]`` (``x is not y``) with an autograd graph to the kernel's tensor hyper-parameters, ``xsg`` and
     ``xg``."""
-    return _KernelCross.apply(coef_tensor(flat, xsg), xsg, xg, [fs for _, fs in flat.terms], param_tensor(flat, xsg))
+    return _KernelCross.apply(flat, coef_tensor(flat, xsg), xsg, xg, param_tensor(flat, xsg))
 
 
 class _KernelDiag(torch.autograd.Function):
     """Differentiable ``k.elwise(x)`` (same points); the backward is the prior-variance term of the rectangular K1-backward."""
 
     @staticmethod
-    def forward(ctx, coefs, xg, structure, params):
-        flat = _flat_of(coefs, structure, xg.shape[0])
+    def forward(ctx, flat, coefs, xg, params):
         ctx.flat, ctx.xg = flat, xg.detach().contiguous()
         return ops.kernel_diag(flat, ctx.xg)
 
@@ -236,16 +231,16 @@ class _KernelDiag(torch.autograd.Function):
     def backward(ctx, g):
         flat, xg = ctx.flat, ctx.xg
         nig = ctx.needs_input_grad
-        ts = torch.zeros(xg.shape[1], _lib.GPK_MAX_TERMS, dtype=xg.dtype, device=xg.device) if nig[0] else None
-        gx = torch.zeros_like(xg) if nig[1] else None
+        ts = torch.zeros(xg.shape[1], _lib.GPK_MAX_TERMS, dtype=xg.dtype, device=xg.device) if nig[1] else None
+        gx = torch.zeros_like(xg) if nig[2] else None
         ps = _param_buf(nig[3], xg.shape[1], xg)
         ops.kernel_cross_bwd(flat, xg, xg, gdiag=g.contiguous(), term_sum=ts, grad_xsg=gx, param_sum=ps)
-        return None if ts is None else ts[:, : len(flat.terms)].sum(0), gx, None, _param_grad(flat, ps)
+        return None, None if ts is None else ts[:, : len(flat.terms)].sum(0), gx, _param_grad(flat, ps)
 
 
 def kernel_diag_grad(flat, xg):
     """``k.elwise(x) [B, n]`` with an autograd graph to the kernel's tensor hyper-parameters and to ``xg``."""
-    return _KernelDiag.apply(coef_tensor(flat, xg), xg, [fs for _, fs in flat.terms], param_tensor(flat, xg))
+    return _KernelDiag.apply(flat, coef_tensor(flat, xg), xg, param_tensor(flat, xg))
 
 
 class _NoGradient(torch.autograd.Function):
@@ -526,11 +521,12 @@ class _ExactPosterior(torch.autograd.Function):
 
 def exact_posterior(spec, coefs_x, xg_x, noise_s, noise_v, ybar, coefs_c, xsg, zg, P=None, params_x=None, params_c=None):
     """``(dot, sq, cov)`` of the exact posterior as ``spec.fwd()`` computes them (an empty tensor for those not formed),
-    differentiable w.r.t. ``K_x``'s coefficients, inputs ``xg_x`` and noise, ``ybar [B, n]``, the cross kernel's coefficients,
-    the test points ``xsg``, the data points ``zg`` (both stretched by the cross kernel's length scales), the prior
-    covariance ``P`` of ``cov`` and the shape parameters of ``K_x``'s and the cross kernel (``params_x``, ``params_c``:
-    :func:`param_tensor`)."""
-    return _ExactPosterior.apply(spec, coefs_x, xg_x, noise_s, noise_v, ybar, coefs_c, xsg, zg, P, params_x, params_c)
+    differentiable w.r.t. ``K_x``'s coefficients, inputs ``xg_x`` and noise (``noise_s``: a float or a tensor; ``noise_v``
+    ``[B, n]`` or None), ``ybar [B, n]``, the cross kernel's coefficients, the test points ``xsg``, the data points ``zg``
+    (both stretched by the cross kernel's length scales), the prior covariance ``P`` of ``cov`` and the shape parameters of
+    ``K_x``'s and the cross kernel (``params_x``, ``params_c``: :func:`param_tensor`)."""
+    return _ExactPosterior.apply(spec, coefs_x, xg_x, _scalar(noise_s, xg_x), noise_v, ybar, coefs_c, xsg, zg, P, params_x,
+                                 params_c)
 
 
 def _posterior_backward(ctx, a, s, gc):

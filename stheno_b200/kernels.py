@@ -1074,9 +1074,8 @@ def _exact_args(post, x):
         return None
     from .autograd import coef_tensor, param_tensor
 
-    coefs_x, ns = K_z.grad_params()
-    return (flat, coefs_x, K_z.xg, ns, K_z.noise_vec, coef_tensor(flat, xsg), xsg, zg, param_tensor(K_z.flat, K_z.xg),
-            param_tensor(flat, xsg))
+    return (flat, coef_tensor(K_z.flat, K_z.xg), K_z.xg, K_z.noise, K_z.noise_vec, coef_tensor(flat, xsg), xsg, zg,
+            param_tensor(K_z.flat, K_z.xg), param_tensor(flat, xsg))
 
 
 def _posterior_call(post, x, fwd, what, *others, mean=False, P=None, cross=None):

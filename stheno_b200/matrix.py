@@ -175,9 +175,8 @@ class KernelDense(Dense):
                 from .autograd import kernel_matrix_grad
 
                 K = kernel_matrix_grad(self.flat, self.xg)
-                nz = self.noise_t if self.noise_t is not None else self.noise_scalar
                 eye = torch.eye(self.n, dtype=K.dtype, device=K.device)
-                K = K + nz * eye
+                K = K + self.noise * eye
                 if self.noise_vec is not None:
                     K = K + torch.diag_embed(self.noise_vec)
             else:
@@ -185,6 +184,11 @@ class KernelDense(Dense):
                                       noise_vec=None if self.noise_vec is None else self.noise_vec.detach())
             self._mat = K.reshape(self.batch_shape + (self.n, self.n))
         return self._mat
+
+    @property
+    def noise(self):
+        """The scalar noise: ``noise_t`` (with its graph) when there is one, else ``noise_scalar``."""
+        return self.noise_scalar if self.noise_t is None else self.noise_t
 
     @property
     def shape(self):
@@ -221,22 +225,9 @@ class KernelDense(Dense):
     def logpdf_grad(self, rhs_t):
         """Differentiable ``logpdf`` ``[B, k]`` w.r.t. kernel scales, length scales / inputs (through ``xg``), shape
         parameters (RQ's alpha), noise and the right-hand sides."""
-        from .autograd import kernel_logpdf, param_tensor
+        from .autograd import kernel_logpdf
 
-        coefs, ns = self.grad_params()
-        structure = [fs for _, fs in self.flat.terms]
-        return kernel_logpdf(coefs, self.xg, ns, self.noise_vec, rhs_t, structure, _B.epsilon,
-                             param_tensor(self.flat, self.xg))
-
-    def grad_params(self):
-        """``(coefs [T], scalar noise [])`` as tensors carrying the graph of those given as tensors that require grad."""
-        from .autograd import coef_tensor
-
-        if self.noise_t is not None:
-            ns = self.noise_t.to(device=self.xg.device, dtype=self.xg.dtype).reshape(())
-        else:
-            ns = torch.tensor(self.noise_scalar, device=self.xg.device, dtype=self.xg.dtype)
-        return coef_tensor(self.flat, self.xg), ns
+        return kernel_logpdf(self.flat, self.xg, self.noise, self.noise_vec, rhs_t, _B.epsilon)
 
 
 class BlockDense(Dense):

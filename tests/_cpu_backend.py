@@ -314,13 +314,13 @@ def install(monkeypatch):
     import sys
 
     import stheno_b200
-    from stheno_b200 import _util, autograd, kernels, matrix
+    from stheno_b200 import _util, autograd, kernels, matrix, pathwise
     from stheno_b200 import random as random_mod
     from stheno_b200.model import observations
 
     me = sys.modules[__name__]
     monkeypatch.setattr(_util, "_device_fn", lambda: torch.device("cpu"))
-    # autograd too (imported here, before the swap): a module first imported while the stand-ins are installed would keep
-    # them after the test, and a GPU test later in the session would run on them
-    for mod in (kernels, matrix, observations, random_mod, autograd, stheno_b200):
+    # autograd and pathwise too (imported here, before the swap): a module first imported while the stand-ins are installed
+    # would keep them after the test, and a GPU test later in the session would run on them
+    for mod in (kernels, matrix, observations, random_mod, autograd, pathwise, stheno_b200):
         monkeypatch.setattr(mod, "ops", me, raising=False)

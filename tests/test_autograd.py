@@ -58,6 +58,47 @@ def test_logpdf_gradients(n, d):
         assert err < tol, (name, err, a.flatten()[:3], b.flatten()[:3])
 
 
+@pytest.mark.parametrize("dtype", [torch.float64, torch.float32])
+def test_kernel_functions_launch_the_callers_descriptor(dtype, monkeypatch):
+    """The differentiable kernel matrix, cross-covariance, diagonal and log-pdf launch the descriptor their caller holds:
+    they build no ``ops.FlatKernel`` of their own, and each value equals, bit for bit, the no-grad launch of that
+    descriptor."""
+    import stheno_b200 as S
+    from stheno_b200 import autograd, ops
+    from stheno_b200.kernels import Input
+
+    g = torch.Generator(device="cuda").manual_seed(3)
+    c = torch.tensor(1.3, device="cuda", dtype=dtype, requires_grad=True)
+    ell = torch.tensor(0.7, device="cuda", dtype=dtype, requires_grad=True)
+    flat, scales = (c * S.EQ()).stretch(ell)._flat()
+    xg = Input(torch.randn(40, 2, device="cuda", dtype=dtype, generator=g)).scaled(scales)
+    zg = Input(torch.randn(24, 2, device="cuda", dtype=dtype, generator=g)).scaled(scales)
+    y = torch.randn(1, 1, 40, device="cuda", dtype=dtype, generator=g)
+    noise, jitter = 0.125, 1e-9
+
+    built = []
+    init = ops.FlatKernel.__init__
+
+    def spy(self, *args, **kwargs):
+        built.append(args)
+        init(self, *args, **kwargs)
+
+    monkeypatch.setattr(ops.FlatKernel, "__init__", spy)
+    got = [autograd.kernel_matrix_grad(flat, xg), autograd.kernel_cross_grad(flat, xg, zg),
+           autograd.kernel_diag_grad(flat, xg)]
+    assert not built
+    got.append(autograd.kernel_logpdf(flat, xg, noise, None, y, jitter))
+    sum(t.sum() for t in got).backward()
+    assert not built
+    assert c.grad is not None and ell.grad is not None
+
+    with torch.no_grad():
+        want = [ops.kernel_matrix(flat, xg), ops.kernel_matrix(flat, xg, zg, same=False), ops.kernel_diag(flat, xg),
+                ops.chol_from_kernel(flat, xg, noise_scalar=noise, jitter=jitter, rhs_t=y, full_precision=True).logpdf()]
+    for name, a, b in zip(("matrix", "cross", "diag", "logpdf"), got, want):
+        assert torch.equal(a.detach(), b), name
+
+
 def test_optimisation_loop_decreases_loss():
     # the shape of readme_example13_optimisation_torch.py:46-53 with plain torch.optim
     import stheno_b200 as S

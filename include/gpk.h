@@ -368,6 +368,21 @@ int gpk_feature_eval_f32(const float* x, int64_t ldx, int64_t n, int32_t d, cons
                          const float* amp, int64_t F, const float* W, int64_t ldw, int32_t num, float* out, int64_t ldo,
                          int32_t accumulate, void* stream);
 
+/* Backward of gpk_feature_eval in x, for the upstream gradient G: [n x num] (ld = ldg); x, omega, b, amp, W as there:
+ *   grad_x[i][e] = (accumulate ? grad_x[i][e] : 0) - sum_j c_ij sin(x_i . omega[j] + b[j]) omega[j][e],
+ *   c_ij = amp[j] sum_s G[i][s] W[s][j],   i < n, e < d;   grad_x: [n x d] (ld = ld).
+ * Neither the n x F features nor c are written to memory: each CTA owns 64 rows and up to 32 dimensions of grad_x (wider
+ * inputs are split over CTAs, each recomputing its rows' phases and c), walks the features in blocks and reduces c over
+ * every sample; both contractions run on the fp64 tensor cores (DMMA) for the fp64 entry point with num >= 8 and by
+ * CUDA-core FMAs otherwise.  Phases and sines as in gpk_feature_eval; the fp32 entry point sums in fp32.  No atomics: the
+ * result is the same bit for bit from run to run.  A row of x or of G holding a NaN gives a NaN row of grad_x. */
+int gpk_feature_eval_bwd_f64(const double* x, int64_t ldx, int64_t n, int32_t d, const double* omega, const double* b,
+                             const double* amp, int64_t F, const double* W, int64_t ldw, int32_t num, const double* G,
+                             int64_t ldg, double* grad_x, int64_t ld, int32_t accumulate, void* stream);
+int gpk_feature_eval_bwd_f32(const float* x, int64_t ldx, int64_t n, int32_t d, const float* omega, const float* b,
+                             const float* amp, int64_t F, const float* W, int64_t ldw, int32_t num, const float* G,
+                             int64_t ldg, float* grad_x, int64_t ld, int32_t accumulate, void* stream);
+
 /* Measurement helper (bench.py): runs a register-resident fp64 tensor-core (DMMA) loop on every SM and returns the
  * achieved TFLOP/s -- the denominator of the fp64 roofline -- or a negative error code.  Synchronises the device. */
 double gpk_probe_dmma_tflops(void);

@@ -62,6 +62,8 @@ _SIGNATURES = {
                               _i32, _ptr, _i64, _ptr, _ptr, _ptr, _i64, "OZ", _ptr],
     "gpk_sparse_rows_bwd": [_i64, _i64, _ptr, _i64, _ptr, _i64, _ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _ptr],
     "gpk_feature_eval": [_ptr, _i64, _i64, _i32, _ptr, _ptr, _ptr, _i64, _ptr, _i64, _i32, _ptr, _i64, _i32, _ptr],
+    "gpk_feature_eval_bwd": [_ptr, _i64, _i64, _i32, _ptr, _ptr, _ptr, _i64, _ptr, _i64, _i32, _ptr, _i64, _ptr, _i64, _i32,
+                             _ptr],
 }
 _PLAIN = {
     "gpk_version": ([], c_int32),

@@ -18,7 +18,7 @@ import torch
 from . import _lib, ops
 
 __all__ = ["kernel_logpdf", "dense_logpdf", "kernel_matrix_grad", "kernel_cross_grad", "kernel_diag_grad", "exact_posterior",
-           "sparse_posterior_marginals", "subspace_cov", "no_gradient"]
+           "sparse_posterior_marginals", "subspace_cov", "no_gradient", "function_sample"]
 
 
 def _bwd_kernel(flat, xg, G, n, param_sum=None):
@@ -629,6 +629,67 @@ def _posterior_backward(ctx, a, s, gc):
         grad_P = grad_P.reshape(ctx.P_shape)
     return (grad_coefs_x, grad_xg_x, grad_ns, grad_nv, grad_y, grad_coefs_c, g_xs, g_z, grad_P, grad_params_x,
             _param_grad(flat_c, ps_c))
+
+
+# ---- pathwise function samples in their inputs ----------------------------------------------------------------------
+#
+# f(x) = m(x) + sum_j (W a)_sj cos(t_j(x)) + t(x) lin + k(x, X) V^T with t = the mapped points and V fixed by the draw:
+#   d/dt   = -sum_j c_ij sin(t_i . omega_j + b_j) omega_j,  c = g (W a)      (gpk_feature_eval_bwd)
+#   d/dk(x*_c, X) = g_c V                                                    (rectangular K1-backward, chunk by chunk)
+# The mean and the linear part pass through unchanged (their graphs are their own); nothing else gets a gradient.
+class _FunctionSample(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, fs, flat, mean, t, lin_part, xsg):
+        ctx.set_materialize_grads(False)
+        ctx.fs, ctx.flat = fs, flat
+        ctx.t, ctx.xsg = t.detach(), None if xsg is None else xsg.detach()
+        return fs.evaluate(mean.detach(), ctx.t, None if lin_part is None else lin_part.detach(), flat, ctx.xsg)
+
+    @staticmethod
+    def backward(ctx, g):
+        _, _, want_m, want_t, want_lin, want_xs = ctx.needs_input_grad
+        if g is None:
+            return (None,) * 6
+        fs, g = ctx.fs, g.contiguous()
+        grad_t = grad_xs = None
+        if want_t:
+            omega, b, amp, W, _ = fs._params(g.dtype)
+            grad_t = ops.feature_eval_bwd(ctx.t, omega, b, amp, W, g)
+        if want_xs:
+            grad_xs = _sample_update_bwd(fs, ctx.flat, ctx.xsg, g)
+        return None, None, g.sum(1, keepdim=True) if want_m else None, grad_t, g if want_lin else None, grad_xs
+
+
+def _sample_update_bwd(fs, flat, xsg, g):
+    """The gradient in ``xsg`` of ``sum g * k(x*, X) V^T``, over the forward's chunks: ``G_c = g_c V`` factored (``u v^T``) for
+    one sample, else formed in one ``chunk x n_pad`` buffer by one GEMM against ``V^T``."""
+    ch = fs._post.K_z.chol()
+    n, num, m = ch.n, fs.num, xsg.shape[2]
+    grad = torch.empty_like(xsg)
+    for a in range(0, m, fs.chunk):
+        c = min(m, a + fs.chunk) - a
+        xs_c = xsg[:, :, a : a + c].contiguous()
+        gx = torch.zeros_like(xs_c)
+        if num == 1:
+            ops.kernel_cross_bwd(flat, xs_c, fs._zg, u=g[a : a + c, 0].reshape(1, c), v=fs.V[0, :1, :n], grad_xsg=gx)
+        else:
+            Vt = fs.V_t()
+            A = torch.zeros(1, ops.round_up(c), Vt.shape[2], dtype=g.dtype, device=g.device)
+            A[0, :c, :num] = g[a : a + c]
+            Gc = ops.gemm_nt(A, Vt)
+            del A
+            ops.kernel_cross_bwd(flat, xs_c, fs._zg, W=Gc, grad_xsg=gx)
+            del Gc
+        grad[:, :, a : a + c] = gx
+    return grad
+
+
+def function_sample(fs, mean, t, lin_part, flat, xsg):
+    """The pathwise sample ``fs`` (:class:`pathwise.FunctionSample`) evaluated from its parts (``FunctionSample._parts``:
+    the prior mean ``[n, 1]``, the feature points ``t [n, d]``, the linear part ``[n, num]`` or None, the update's cross
+    kernel ``flat`` and pre-stretched points ``xsg [G, 1, n, d]``, or None, None for a prior) by the launches of the no-grad
+    evaluation, differentiable w.r.t. ``mean``, ``t``, ``lin_part`` and ``xsg``.  ``[n, num]``."""
+    return _FunctionSample.apply(fs, flat, mean, t, lin_part, xsg)
 
 
 def _solved_rows(ch, flat_c, xs_c, zg):

@@ -248,6 +248,35 @@ def feature_eval(x, omega, b, amp, W, out=None, chunk=1 << 20):
     return out
 
 
+def feature_eval_bwd(x, omega, b, amp, W, G, out=None, chunk=1 << 20):
+    """The gradient in ``x`` of ``sum_is G[i, s] feature_eval(x, omega, b, amp, W)[i, s]`` (``gpk_feature_eval_bwd``):
+    ``-sum_j c_ij sin(x_i . omega_j + b_j) omega_j`` with ``c_ij = amp_j sum_s G[i, s] W[s, j]``; ``G [n, num]`` -> ``[n, d]``.
+    With ``out`` (a ``[n, d]`` tensor with a unit inner stride) the gradient is added to it, else a new tensor is returned.
+    Rows are launched ``chunk`` at a time; neither the ``n x F`` features nor ``c`` are held."""
+    _require_cuda(x, omega, b, amp, W, G, out)
+    x, omega, b, amp, W, G = [t.contiguous() for t in (x, omega, b, amp, W, G)]
+    n, d = x.shape
+    F, num = omega.shape[0], W.shape[0]
+    if omega.shape[1] != d or b.shape != (F,) or amp.shape != (F,) or W.shape[1] != F or G.shape != (n, num):
+        raise ValueError("feature_eval_bwd: shapes do not match")
+    if any(t.dtype != x.dtype for t in (omega, b, amp, W, G, out) if t is not None):
+        raise TypeError("feature_eval_bwd: x, omega, b, amp, W, G and out must share one dtype")
+    accumulate = out is not None
+    if out is None:
+        out = (torch.zeros if F == 0 else torch.empty)(n, d, device=x.device, dtype=x.dtype)
+    elif out.shape != (n, d) or out.stride(1) != 1:
+        raise ValueError("feature_eval_bwd: out must be [n, d] with a unit inner stride")
+    if F == 0:
+        return out
+    fn = _fn("gpk_feature_eval_bwd", x.dtype)
+    for a in range(0, n, chunk):
+        c = min(n, a + chunk) - a
+        rc = fn(_ptr(x[a]), d, c, d, _ptr(omega), _ptr(b), _ptr(amp), F, _ptr(W), F, num, _ptr(G[a]), num, _ptr(out[a]),
+                out.stride(0), 1 if accumulate else 0, _stream())
+        check(rc, "gpk_feature_eval_bwd")
+    return out
+
+
 def _pad_copy(src, dst, rows, cols, rows_pad, cols_pad, diag_add, pad_identity):
     if src.stride(2) != 1:
         src = src.contiguous()

@@ -6,7 +6,9 @@ output, the (mapped) points and one ``chunk x n_pad`` block of K1 rows of the up
     posterior:  f(x)  = f~(x) + k(x, X) V^T,   V = K^-1 (y - f~(X) - eps),   K = k(X, X) + Sigma_noise + B.epsilon I
 
 The cosine features run in ``gpk_feature_eval`` (``csrc/sample_fn.cu``), which never holds the n x F feature matrix; the
-update reuses the factor of ``K`` that ``Observations.K_x`` keeps, the K1 rows and the tensor-core GEMM.
+update reuses the factor of ``K`` that ``Observations.K_x`` keeps, the K1 rows and the tensor-core GEMM.  A sample is
+differentiable in its evaluation points only (``autograd.function_sample``): ``gpk_feature_eval_bwd`` differentiates the
+features, the rectangular K1-backward the update.
 
 Spectral measures of the unit-length-scale factors of ``include/gpk.h``:
     EQ ``exp(-r^2 / 2)``:                 omega ~ N(0, I)
@@ -23,7 +25,7 @@ from . import _util, ops
 from . import matrix as M
 from ._util import from_dev
 from .kernels import (DerivativeKernel, FunctionScaledKernel, MappedKernel, PosteriorKernel, PosteriorMean, SubspaceKernel,
-                      _children, _grad_tensors, _is_multi, _same_map, as_input, k1_block)
+                      _children, _grad_tensors, _is_multi, _same_map, as_input, k1_block, map_output_grads)
 
 __all__ = ["FunctionSample"]
 
@@ -165,6 +167,7 @@ class FunctionSample:
         self._gen = torch.Generator(device=self.device).manual_seed(seed)
         self.omega = None
         self.eps = self.V = None
+        self._zg = self._Vt = None
         if self._post is not None:
             with torch.no_grad():
                 self._condition()
@@ -197,8 +200,9 @@ class FunctionSample:
                                                                               self.linear)]
         return self._cast[dtype]
 
-    def _prior(self, xi):
-        """``f~`` at the points of the :class:`Input` ``xi``: ``[n, num]``."""
+    def _feature_points(self, xi):
+        """The points of the :class:`Input` ``xi`` the features read (through the kernel's input maps, with their graph),
+        drawing the features at the first call."""
         _, _, xm, _ = k1_block(self.kernel, xi, through_maps=True, zero=True)
         t = xm.t
         if self.omega is None:
@@ -206,13 +210,44 @@ class FunctionSample:
         elif t.shape[-1] != self.omega.shape[1]:
             raise ValueError(f"this function sample was drawn for inputs of dimension {self.omega.shape[1]} (after the "
                              f"kernel's input maps), not {t.shape[-1]}")
-        omega, b, amp, W, lin = self._params(t.dtype)
-        out = self.mean.dev(xi).reshape(-1, 1).expand(-1, self.num).contiguous()
+        return t
+
+    def _parts(self, xi, update=True):
+        """``(mean [n, 1], t, t lin or None, flat, xsg)``: what :meth:`evaluate` reads at the points of ``xi``, each with its
+        graph to ``xi``: the prior mean, the feature points ``t``, the linear part, and for a posterior (and ``update``) the
+        update's cross kernel and the points it reads, mapped and pre-stretched ``[G, 1, n, d]`` (else None, None).  The
+        length scales stretch without a graph: a sample is differentiated in its inputs only."""
+        t = self._feature_points(xi)
+        lin = self._params(t.dtype)[4]
+        flat = xsg = None
+        if update and self._post is not None:
+            post = self._post
+            flat, scales, zm, xm = k1_block(post.k_zi, post.z, xi, through_maps=True)
+            scales = [s.detach() if isinstance(s, torch.Tensor) else s for s in scales]
+            if self._zg is None:
+                with torch.no_grad():
+                    self._zg = zm.scaled(scales)
+            xsg = xm.scaled(scales)
+        return self.mean.dev(xi).reshape(-1, 1), t, None if lin is None else t @ lin, flat, xsg
+
+    def evaluate(self, mean, t, lin_part, flat, xsg):
+        """The launches of an evaluation from :meth:`_parts` (without graphs): the prior mean, one feature launch over every
+        point (the kernel holds no n x F buffer), the linear part, then the update, chunked (it holds a chunk x n_pad block of
+        K1 rows).  ``[n, num]``."""
+        omega, b, amp, W, _ = self._params(t.dtype)
+        out = mean.expand(-1, self.num).contiguous()
         if omega.shape[0]:
             ops.feature_eval(t, omega, b, amp, W, out=out)
-        if lin is not None:
-            out += t @ lin
+        if lin_part is not None:
+            out += lin_part
+        if xsg is not None:
+            for a in range(0, t.shape[0], self.chunk):
+                out[a : a + self.chunk] += self._update(flat, xsg[:, :, a : a + self.chunk])
         return out
+
+    def _prior(self, xi):
+        """``f~`` at the points of the :class:`Input` ``xi``: ``[n, num]``."""
+        return self.evaluate(*self._parts(xi, update=False))
 
     # ---- the update ----------------------------------------------------------------------------------------------------
     def _condition(self):
@@ -233,23 +268,25 @@ class FunctionSample:
         ch.solve_rows_(V)
         ch.solve_rows_t_(V)
         self.V = V
-        self._zg = None
+        self._zg = self._Vt = None
 
-    def _update(self, xi):
-        """``k(x, X) V^T`` at the points of ``xi``: ``[n, num]``."""
-        post = self._post
-        ch = post.K_z.chol()
-        flat, scales, zm, xm = k1_block(post.k_zi, post.z, xi, through_maps=True)
-        if self._zg is None:
-            self._zg = zm.scaled(scales)
-        rows = ops.kernel_rows_padded(flat, xm.scaled(scales), self._zg, ch)
+    def _update(self, flat, xsg):
+        """``k(x, X) V^T`` at the pre-stretched points ``xsg [G, 1, c, d]`` of one chunk: ``[c, num]``."""
+        ch = self._post.K_z.chol()
+        rows = ops.kernel_rows_padded(flat, xsg, self._zg, ch)
         # rows V^T has one 128-column tile for up to 128 samples: split the n_pad-long reduction into `s` batched partial
         # products so that s times as many CTAs share it (each part a multiple of 32 long, as the fp32 tensor-core GEMM needs)
         s = 8 if ch.n_pad % 256 == 0 else 4
         k, c_pad = ch.n_pad // s, rows.shape[1]
         A = rows[0].view(c_pad, s, k).transpose(0, 1)
         Bm = self.V[0].view(self.V.shape[1], s, k).transpose(0, 1)
-        return ops.gemm_nt(A, Bm).sum(0)[: xi.n, : self.num]
+        return ops.gemm_nt(A, Bm).sum(0)[: xsg.shape[2], : self.num]
+
+    def V_t(self):
+        """``V^T`` padded, ``[1, n_pad, num_pad]``, formed once (the backward of the update reads it)."""
+        if self._Vt is None:
+            self._Vt = ops.transpose(self.V, self.V.shape[1], self.V.shape[2])
+        return self._Vt
 
     # ---- evaluation ----------------------------------------------------------------------------------------------------
     def __call__(self, x):
@@ -261,15 +298,34 @@ class FunctionSample:
         if xi.batch_shape:
             raise ValueError("function sampling does not cover batched inputs")
         dtype = self.V.dtype if self.V is not None else xi.t.dtype
-        ts = _grad_tensors(self._gp_mean, self._gp_kernel, xi)
-        with torch.no_grad():
-            xd = as_input(xi.t.detach().to(dtype))
-            out = self._prior(xd)  # one feature launch over every point: the kernel holds no n x F buffer
-            if self._post is not None:  # the update holds a chunk x n_pad block of K1 rows: chunked
-                for a in range(0, xd.n, self.chunk):
-                    out[a : a + self.chunk] += self._update(as_input(xd.t[a : a + self.chunk]))
+        xd = as_input(xi.t.detach().to(dtype))
+        ts = _grad_tensors(self._gp_mean, self._gp_kernel, xi) + self._hidden_grads(xd)
+        if any(t is xi.t for t in ts):
+            from .autograd import function_sample
+
+            parts = self._parts(as_input(xi.t.to(dtype)))
+            out = function_sample(self, *parts)
+        else:
+            with torch.no_grad():
+                out = self.evaluate(*self._parts(xd))
+        ts = [t for t in ts if t is not xi.t]
         if ts:
+            # the value's other inputs (hyper-parameters, observations, maps' and means' parameters) get no gradient: a node
+            # on a branch that only they feed raises, so a backward to the evaluation points alone still works
             from .autograd import no_gradient
 
-            out = no_gradient("function sampling", out, ts)
+            out = out + no_gradient("function sampling", out.new_zeros(()), ts)
         return from_dev(out, xi.origin)
+
+    def _hidden_grads(self, xd):
+        """The tensors that require grad hidden in the closure of a ``transform`` of the kernel or of a mean function: the
+        maps' and the mean's outputs at the detached points ``xd`` and, for a posterior, at the data points."""
+        if not torch.is_grad_enabled():
+            return []
+        out = []
+        for p in [xd] + ([self._post.z] if self._post is not None else []):
+            out += map_output_grads(self.kernel, p, p)
+            m = self.mean.dev(p)
+            if m.requires_grad:
+                out.append(m)
+        return out

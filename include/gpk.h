@@ -383,6 +383,23 @@ int gpk_feature_eval_bwd_f32(const float* x, int64_t ldx, int64_t n, int32_t d, 
                              const float* amp, int64_t F, const float* W, int64_t ldw, int32_t num, const float* G,
                              int64_t ldg, float* grad_x, int64_t ld, int32_t accumulate, void* stream);
 
+/* Leave-one-out finish (stheno_b200/random.py, Normal.loo_marginals / loo_logpdf) of y ~ N(m, Sigma), r = y - m, from
+ * c = diag Sigma^-1 ([batch][n], batch stride c_bstride), alpha = Sigma^-1 r ([batch][k][n], ld lda, batch stride a_bstride)
+ * and r ([batch][k][n], ld ldr, batch stride r_bstride; read only for mu).  Without g (NULL), into contiguous outputs:
+ *   mu[b][c][i] = r_ci - alpha_ci / c_i   (the LOO mean of y_ci minus m_i),   var[b][i] = 1 / c_i,
+ *   lp[b][c] = sum_i (-1/2 log 2 pi + 1/2 log c_i - 1/2 alpha_ci^2 / c_i)
+ * With g ([batch][k], the upstream gradient of lp) it forms the backward weights instead:
+ *   P[b][i] = sum_c g_c (1 + alpha_ci^2 / c_i) / (2 c_i),   q[b][c][i] = g_c alpha_ci / c_i
+ * so that d(sum_c g_c lp_c)/dSigma = -Sigma^-1 diag(P) Sigma^-1 + 1/2 sum_c (beta_c alpha_c^T + alpha_c beta_c^T) and
+ * d/dr_c = -beta_c with beta_c = Sigma^-1 q_c.  Every output may be NULL (not formed).  One CTA per column sums lp in a
+ * fixed order: the value is the same bit for bit from run to run.  fp64 arithmetic and sums in both precisions. */
+int gpk_loo_finish_f64(const double* c, int64_t c_bstride, const double* alpha, int64_t lda, int64_t a_bstride,
+                       const double* r, int64_t ldr, int64_t r_bstride, int64_t n, int32_t k, const double* g, double* mu,
+                       double* var, double* lp, double* P, double* q, int32_t batch, void* stream);
+int gpk_loo_finish_f32(const float* c, int64_t c_bstride, const float* alpha, int64_t lda, int64_t a_bstride, const float* r,
+                       int64_t ldr, int64_t r_bstride, int64_t n, int32_t k, const float* g, float* mu, float* var,
+                       float* lp, float* P, float* q, int32_t batch, void* stream);
+
 /* Measurement helper (bench.py): runs a register-resident fp64 tensor-core (DMMA) loop on every SM and returns the
  * achieved TFLOP/s -- the denominator of the fp64 roofline -- or a negative error code.  Synchronises the device. */
 double gpk_probe_dmma_tflops(void);

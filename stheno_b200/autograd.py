@@ -17,7 +17,7 @@ import torch
 
 from . import _lib, ops
 
-__all__ = ["kernel_logpdf", "dense_logpdf", "kernel_matrix_grad", "kernel_cross_grad", "kernel_diag_grad", "exact_posterior",
+__all__ = ["kernel_logpdf", "dense_logpdf", "kernel_loo", "dense_loo", "kernel_matrix_grad", "kernel_cross_grad", "kernel_diag_grad", "exact_posterior",
            "sparse_posterior_marginals", "subspace_cov", "no_gradient", "function_sample"]
 
 
@@ -97,24 +97,118 @@ def _alpha_and_G_impl(ch, g):
     arows[:, :k, :n] = ch.rhs_half()
     ch.solve_rows_t_(arows)
     alpha = arows[:, :k, :n]
-    V = torch.zeros(Bn, n_pad, n_pad, dtype=dtype, device=dev)
-    V.diagonal(dim1=1, dim2=2).fill_(1.0)
-    ch.solve_rows_(V)  # rows (L^-1 e_r)^T, i.e. V = L^-T ; K^-1 = V V^T
-    Gm = torch.empty(Bn, n_pad, n_pad, dtype=dtype, device=dev)
+    Gm = _inverse_lower(ch, -0.5)
     kp = ops.round_up(k, 16)
     for b in range(Bn):
         # the weight sum(g_c) scales the product on the device: reading it on the host would make the backward wait for
         # everything enqueued before it on the stream
-        ops.gemm_nt(V[b : b + 1], V[b : b + 1], Gm[b : b + 1], alpha=-0.5, beta=0.0, lower=True)
         Gm[b].mul_(g[b].sum())
         A = torch.zeros(1, n_pad, kp, dtype=dtype, device=dev)
         Bm = torch.zeros(1, n_pad, kp, dtype=dtype, device=dev)
         A[0, :n, :k] = (alpha[b] * (0.5 * g[b]).unsqueeze(-1)).t()
         Bm[0, :n, :k] = alpha[b].t()
         ops.gemm_nt(A, Bm, Gm[b : b + 1], alpha=1.0, beta=1.0, lower=True)
-    del V
     ops.symmetrize_(Gm, n_pad)
     return alpha, Gm
+
+
+def _inverse_lower(ch, scale):
+    """``scale K^-1`` on the lower 128-tiles of a new padded ``[B, n_pad, n_pad]`` tensor (the upper ones are left
+    unwritten): ``V = L^-T`` by one solve of the identity, then ``V V^T`` by one lower-tile product per batch member."""
+    Bn, n_pad = ch.batch, ch.n_pad
+    V = torch.zeros(Bn, n_pad, n_pad, dtype=ch.dtype, device=ch.device)
+    V.diagonal(dim1=1, dim2=2).fill_(1.0)
+    ch.solve_rows_(V)  # rows (L^-1 e_r)^T, i.e. V = L^-T ; K^-1 = V V^T
+    out = torch.empty(Bn, n_pad, n_pad, dtype=ch.dtype, device=ch.device)
+    for b in range(Bn):
+        ops.gemm_nt(V[b : b + 1], V[b : b + 1], out[b : b + 1], alpha=scale, beta=0.0, lower=True)
+    return out
+
+
+# ---- leave-one-out log densities ------------------------------------------------------------------------------------------
+#
+# c = diag K^-1, alpha_c = K^-1 r_c, LOO_c = sum_i (-1/2 log 2 pi + 1/2 log c_i - 1/2 alpha_ci^2 / c_i).  For L = sum_c g_c LOO_c,
+# with the weights P, q of gpk_loo_finish and beta_c = K^-1 q_c:
+#   dL/dK   = -K^-1 diag(P) K^-1 + 1/2 sum_c (beta_c alpha_c^T + alpha_c beta_c^T)
+#   dL/dr_c = -beta_c
+def _loo_G(ch, alpha, c, g):
+    """``(dL/dK [B, n_pad, n_pad] symmetric, beta [B, k, n])`` from the factor, ``alpha``, ``c`` and the upstream ``g [B, k]``.
+    At most three ``n_pad^2`` buffers at once: ``V`` and ``K^-1``, then ``K^-1``, its column-scaled copy and ``dL/dK``."""
+    Bn, n, n_pad, k = ch.batch, ch.n, ch.n_pad, alpha.shape[1]
+    P, q = ops.loo_finish(c, alpha, g=g.contiguous())
+    Kinv = _inverse_lower(ch, 1.0)
+    ops.symmetrize_(Kinv, n_pad)
+    Gm = torch.empty_like(Kinv)
+    Pp = torch.zeros(Bn, 1, n_pad, dtype=ch.dtype, device=ch.device)
+    Pp[:, 0, :n] = P
+    for b in range(Bn):
+        ops.gemm_nt(Kinv[b : b + 1] * Pp[b : b + 1], Kinv[b : b + 1], Gm[b : b + 1], alpha=-1.0, beta=0.0, lower=True)
+    del Kinv
+    beta = ch.full_solve(q)
+    kp = ops.round_up(2 * k, 16)
+    A = torch.zeros(Bn, n_pad, kp, dtype=ch.dtype, device=ch.device)
+    Bm = torch.zeros(Bn, n_pad, kp, dtype=ch.dtype, device=ch.device)
+    A[:, :n, :k], A[:, :n, k : 2 * k] = beta.transpose(1, 2), alpha.transpose(1, 2)
+    Bm[:, :n, :k], Bm[:, :n, k : 2 * k] = alpha.transpose(1, 2), beta.transpose(1, 2)
+    for b in range(Bn):
+        ops.gemm_nt(A[b : b + 1], Bm[b : b + 1], Gm[b : b + 1], alpha=0.5, beta=1.0, lower=True)
+    ops.symmetrize_(Gm, n_pad)
+    return Gm, beta
+
+
+class _KernelLoo(torch.autograd.Function):
+    """The summed leave-one-out log densities ``[B, k]`` of ``N(0, k(x, x) + noise + jitter I)`` at ``rhs_t``; arguments as
+    :class:`_KernelLogpdf`'s.  The forward runs the launches of the no-grad route (``Chol.loo``)."""
+
+    @staticmethod
+    def forward(ctx, flat, coefs, xg, noise_scalar, noise_vec, rhs_t, jitter, params):
+        ch = ops.chol_from_kernel(flat, xg.detach().contiguous(), noise_scalar=float(noise_scalar),
+                                  noise_vec=None if noise_vec is None else noise_vec.detach(), jitter=jitter,
+                                  rhs_t=rhs_t.detach(), full_precision=True)
+        _, _, lp, alpha, c = ch.loo(rhs_t.detach(), want_mean=False)
+        ctx.ch, ctx.flat, ctx.alpha, ctx.c = ch, flat, alpha, c
+        ctx.xg = xg.detach().contiguous()
+        ctx.has_nv = noise_vec is not None
+        return lp
+
+    @staticmethod
+    def backward(ctx, g):
+        ch, flat, xg = ctx.ch, ctx.flat, ctx.xg
+        Gm, beta = _loo_G(ch, ctx.alpha, ctx.c, g)
+        ps = _param_buf(ctx.needs_input_grad[7], xg.shape[1], xg)
+        term_sum, grad_xg, diag = _bwd_kernel(flat, xg, Gm, ch.n, ps)
+        del Gm
+        grad_coefs = term_sum[:, : len(flat.terms)].sum(0)
+        grad_nv = diag if ctx.has_nv else None
+        return None, grad_coefs, grad_xg, diag.sum(), grad_nv, -beta, None, _param_grad(flat, ps)
+
+
+def kernel_loo(flat, xg, noise_scalar, noise_vec, rhs_t, jitter):
+    """Differentiable summed leave-one-out log densities ``[B, k]``; arguments and gradients as :func:`kernel_logpdf`'s."""
+    return _KernelLoo.apply(flat, coef_tensor(flat, xg), xg, _scalar(noise_scalar, xg), noise_vec, rhs_t, jitter,
+                            param_tensor(flat, xg))
+
+
+class _DenseLoo(torch.autograd.Function):
+    """:class:`_KernelLoo` for an explicit dense ``K [B, n, n]`` (+ ``jitter I``), with a gradient w.r.t. ``K`` itself."""
+
+    @staticmethod
+    def forward(ctx, K, rhs_t, jitter):
+        ch = ops.chol_from_dense(K.detach(), jitter=jitter, rhs_t=rhs_t.detach())
+        _, _, lp, alpha, c = ch.loo(rhs_t.detach(), want_mean=False)
+        ctx.ch, ctx.alpha, ctx.c = ch, alpha, c
+        return lp
+
+    @staticmethod
+    def backward(ctx, g):
+        ch = ctx.ch
+        Gm, beta = _loo_G(ch, ctx.alpha, ctx.c, g)
+        n = ch.n
+        return Gm[:, :n, :n].contiguous(), -beta, None
+
+
+def dense_loo(K, rhs_t, jitter):
+    return _DenseLoo.apply(K, rhs_t, jitter)
 
 
 class _DenseLogpdf(torch.autograd.Function):

@@ -229,6 +229,19 @@ class KernelDense(Dense):
 
         return kernel_logpdf(self.flat, self.xg, self.noise, self.noise_vec, rhs_t, _B.epsilon)
 
+    def loo_chol(self, rhs_t):
+        """A new full-precision factor of ``self + B.epsilon I`` with ``rhs_t`` fused, for element-wise leave-one-out
+        quantities (the cached factor may be a 7-slice one)."""
+        return ops.chol_from_kernel(self.flat, self.xg.detach(), noise_scalar=self.noise_scalar,
+                                    noise_vec=None if self.noise_vec is None else self.noise_vec.detach(), jitter=_B.epsilon,
+                                    rhs_t=rhs_t, full_precision=True)
+
+    def loo_grad(self, rhs_t):
+        """Differentiable summed leave-one-out log densities ``[B, k]``, with the gradients of :meth:`logpdf_grad`."""
+        from .autograd import kernel_loo
+
+        return kernel_loo(self.flat, self.xg, self.noise, self.noise_vec, rhs_t, _B.epsilon)
+
 
 class BlockDense(Dense):
     """A square grid of blocks ``[[K_ij]]`` (the joint covariance of several processes, ``stheno/mo/input.py:7-19`` /

@@ -465,6 +465,42 @@ class Chol:
             gemm_nt(Bt[:, :, m:b], L21t, Bt[:, :, p0:p1], alpha=-1.0, beta=1.0)
         self._solve_t_block(Bt, a, m, leaf, panel)  # X1 L11 = B1
 
+    def inverse_diag(self, chunk=2048):
+        """``diag (L L^T)^-1`` ``[B, n]``: the squared norms of the rows of ``L^-T``.  Row ``r`` of ``L^-T`` is
+        ``(L^-1 e_r)^T``, zero before column ``r``, so a chunk of identity rows from a 128-aligned ``r0`` is solved against
+        the trailing factor ``L[r0:, r0:]`` alone: ``n^3 / 3`` flops in all and one ``[B, chunk, n_pad]`` buffer, never the
+        ``n_pad^2`` inverse."""
+        _require_cuda(self.W)
+        Lp, n, n_pad, batch = self.L_padded(), self.n, self.n_pad, self.batch
+        chunk = min(round_up(chunk), n_pad)
+        out = torch.empty(batch, n, device=self.device, dtype=self.dtype)
+        buf = torch.empty(batch, chunk, n_pad, device=self.device, dtype=self.dtype)
+        fn = _fn("gpk_trsm_right", self.dtype)
+        for r0 in range(0, n, chunk):
+            rows, m = min(chunk, n_pad - r0), n_pad - r0
+            L, X = Lp[:, r0:, r0:], buf[:, :rows, :m]
+            X.zero_()
+            X.diagonal(dim1=1, dim2=2).fill_(1.0)
+            em = _emulation(self.dtype, self.device, lambda lib, s: lib.gpk_trsm_right_oz_ws_bytes(m, rows, s) if batch == 1 else 0)
+            rc = fn(_ptr(L), L.stride(1), L.stride(0), m, _ptr(X), X.stride(1), X.stride(0), rows, batch, *em, _stream())
+            check(rc, "gpk_trsm_right")
+            r1 = min(n, r0 + rows)
+            out[:, r0:r1] = row_dot_sq(X, r1 - r0, m, want_dot=False)[1]
+        return out
+
+    def loo(self, r, want_mean=True):
+        """Leave-one-out quantities of ``N(0, L L^T)`` at the fused right-hand sides ``r [B, k, n]`` (the rows this factor
+        was built with): ``(mean [B, k, n] (the LOO mean minus the prior mean; None without want_mean), var [B, n],
+        lp [B, k], alpha [B, k, n], c [B, n])`` with ``alpha = K^-1 r`` and ``c = diag K^-1`` (:func:`loo_finish`)."""
+        k, n = self.k, self.n
+        arows = self.new_rows(k)
+        arows[:, :k, :n] = self.rhs_half()
+        self.solve_rows_t_(arows)
+        alpha = arows[:, :k, :n]
+        c = self.inverse_diag()
+        mean, var, lp = loo_finish(c, alpha, r, want_mean=want_mean)
+        return mean, var, lp, alpha, c
+
     def half_solve(self, bt):
         """``bt [B, m, n]`` (rows = right-hand sides) -> ``(L^-1 b)^T [B, m, n]``."""
         m = bt.shape[1]
@@ -481,6 +517,39 @@ class Chol:
         self.solve_rows_(buf)
         self.solve_rows_t_(buf)
         return buf[:, :m, : self.n]
+
+
+def loo_finish(c, alpha, r=None, g=None, *, want_mean=True, want_var=True, want_lp=True):
+    """``gpk_loo_finish`` on ``c [B, n]`` (``diag K^-1``), ``alpha [B, k, n]`` (``K^-1 r``, rows with a unit inner stride)
+    and ``r [B, k, n]``.  Without ``g``: ``(mean [B, k, n], var [B, n], lp [B, k])`` with ``mean = r - alpha / c``,
+    ``var = 1 / c`` and ``lp`` the summed leave-one-out log densities (None for those not wanted).  With the upstream
+    gradient ``g [B, k]`` of ``lp``: the backward weights ``(P [B, n], q [B, k, n])``."""
+    _require_cuda(c, alpha, r, g)
+    Bn, k, n = alpha.shape
+    if c.shape != (Bn, n) or (r is not None and r.shape != (Bn, k, n)) or (g is not None and g.shape != (Bn, k)):
+        raise ValueError("loo_finish: shapes do not match")
+    if c.stride(1) != 1:
+        c = c.contiguous()
+    if alpha.stride(2) != 1:
+        alpha = alpha.contiguous()
+    if r is not None and r.stride(2) != 1:
+        r = r.contiguous()
+    new = lambda *shape: torch.empty(*shape, device=c.device, dtype=c.dtype)  # noqa: E731
+    if g is not None:
+        outs = (None, None, None, new(Bn, n), new(Bn, k, n))
+        g = g.contiguous()
+    else:
+        if want_mean and r is None:
+            raise ValueError("loo_finish: the mean needs r")
+        outs = (new(Bn, k, n) if want_mean else None, new(Bn, n) if want_var else None, new(Bn, k) if want_lp else None,
+                None, None)
+    ld = lambda t: t.stride(1) if k > 1 else n  # noqa: E731  (a contiguous single row may report any row stride)
+    rc = _fn("gpk_loo_finish", c.dtype)(
+        _ptr(c), c.stride(0), _ptr(alpha), ld(alpha), alpha.stride(0), _ptr(r), ld(r) if r is not None else 0,
+        r.stride(0) if r is not None else 0, n, k, _ptr(g), *[_ptr(t) for t in outs], Bn, _stream(),
+    )
+    check(rc, "gpk_loo_finish")
+    return outs[3:] if g is not None else outs[:3]
 
 
 def _new_workspace(B, n, k, device, dtype, rhs_t):

@@ -72,6 +72,34 @@ class _NanFlag:
         return bool(self.cell.item())
 
 
+def _loo_structured(var, rhs_t):
+    """``(c [B, n], alpha [B, k, n])`` of a Diagonal (``c = 1 / d``) or Woodbury (``D + U U^T``: inversion lemma, ``O(n r^2)``)
+    covariance in differentiable torch ops, with the Schur complement regularised by ``B.epsilon`` as in the Woodbury log-pdf."""
+    n = rhs_t.shape[-1]
+    if isinstance(var, M.Diagonal):
+        d = var.diag.reshape(-1, n)
+        return 1.0 / d, rhs_t / d.unsqueeze(1)
+    U, d = var.lr.left, var.diag_m.diag
+    U3 = U.reshape((-1,) + tuple(U.shape[-2:]))
+    r = U3.shape[-1]
+    d3 = d.reshape(-1, n)
+    Ud = U3 / d3.unsqueeze(-1)  # D^-1 U
+    S = torch.eye(r, dtype=U.dtype, device=U.device) + U3.transpose(1, 2) @ Ud
+    L = torch.linalg.cholesky(S + B.epsilon * torch.eye(r, dtype=U.dtype, device=U.device))
+    H = torch.linalg.solve_triangular(L, Ud.transpose(1, 2), upper=False)  # [B, r, n]: L^-1 U^T D^-1
+    c = 1.0 / d3 - (H * H).sum(1)
+    h = H @ rhs_t.transpose(1, 2)  # [B, r, k]
+    alpha = rhs_t / d3.unsqueeze(1) - (H.transpose(1, 2) @ h).transpose(1, 2)
+    return c, alpha
+
+
+def _loo_torch(c, alpha, r):
+    """``gpk_loo_finish``'s forward in differentiable torch ops: ``(mean [B, k, n], var [B, n], lp [B, k])``."""
+    s = alpha / c.unsqueeze(1)
+    lp = 0.5 * ((torch.log(c).unsqueeze(1) - alpha * s).sum(-1) - c.shape[-1] * B.log_2_pi)
+    return r - s, 1.0 / c, lp
+
+
 class Normal(RandomVector):
     """``Normal(mean, var)``, ``Normal(var)`` or the lazy form ``Normal(mean_fn, var_fn, var_diag=..., mean_var=...,
     mean_var_diag=...)`` whose constructors return DEVICE tensors / matrices (``stheno/random.py:56-94``)."""
@@ -280,6 +308,85 @@ class Normal(RandomVector):
         avail = ~nan
         sub = Normal(self._mean_dev()[avail], M.submatrix(var, avail), origin=self._origin)
         return sub.logpdf(from_dev(xd[avail], out_origin))
+
+    # ---- leave-one-out predictive distributions (model checking, LOO cross-validation) --------------------------------
+    def loo_marginals(self, x):
+        """Mean and variance of every ``x_i`` given all the other entries of its column: ``(n,)``/``(n, 1)`` -> ``(n,)``
+        and ``(n,)``, ``(n, k)`` -> ``(n, k)`` and ``(n,)`` (the variance does not depend on ``x``), batched ``(B, n, 1)``
+        -> ``(B, n)`` and ``(B, n)``.  NaN entries of a single column are missing: the others are predicted from the
+        observed ones, and missing positions get NaN.  With ``Sigma = var + B.epsilon I``, ``c = diag Sigma^-1`` and
+        ``alpha = Sigma^-1 (x - mean)``: mean ``x_i - alpha_i / c_i``, variance ``1 / c_i``.  Gradients flow through
+        diagonal and Woodbury covariances only; elsewhere a backward through these values raises."""
+        return self._loo(x, marginals=True)
+
+    def loo_logpdf(self, x):
+        """``sum_i log p(x_i | x_-i)``, the leave-one-out log predictive density, with the output shapes of
+        :meth:`logpdf` and its missing-data rule.  Differentiable like :meth:`logpdf`: every route has a gradient, the
+        kernel-matrix one an analytic one on the GPU."""
+        return self._loo(x, marginals=False)
+
+    def _loo(self, x, marginals):
+        out_origin = origin_of(x) if self._origin is None else self._origin
+        var = self._var_dev()
+        xd = uprank(to_dev(x, None)).to(var.dtype)
+        pending = None
+        if xd.dim() == 2 and xd.shape[1] == 1:  # missing data, detected as in logpdf
+            if isinstance(x, torch.Tensor) and x.is_cuda:
+                if _allow_missing:
+                    pending = _NanFlag(xd)
+            else:
+                host = x.detach().numpy() if isinstance(x, torch.Tensor) else np.asarray(x, dtype=float)
+                if np.isnan(host).any():
+                    return self._loo_missing(xd, marginals, out_origin)
+        n = var.shape[-1]
+        diff = xd if self.mean_is_zero else xd - self._mean_dev()
+        d3, bs = batch_flatten(diff, 2)
+        rhs_t = d3.transpose(1, 2).contiguous()  # [B, k, n]
+        if isinstance(var, (M.Diagonal, M.Woodbury)):
+            c, alpha = _loo_structured(var, rhs_t)
+            mean_r, v, lp = _loo_torch(c, alpha, rhs_t)
+        else:
+            if isinstance(var, M.LowRank):
+                var = M.Dense(var.dev, var.origin)
+            ts = _grad_tensors(var, rhs_t)  # walks the blocks of a BlockDense: never materialises it
+            mean_r = v = None
+            if ts and not marginals and isinstance(var, M.KernelDense):
+                lp = var.loo_grad(rhs_t)
+            elif ts and not marginals:
+                from .autograd import dense_loo
+
+                K3, _ = batch_flatten(var.dev, 2)
+                lp = dense_loo(K3, rhs_t, B.epsilon)  # gradient w.r.t. the assembled covariance itself
+            else:
+                ch = var.loo_chol(rhs_t.detach()) if isinstance(var, M.KernelDense) else var._factorize(rhs_t.detach())
+                mean_r, v, lp, _, _ = ch.loo(rhs_t.detach(), want_mean=marginals)
+                if ts:  # raw-pointer values: a gradient through them would be silently wrong
+                    from .autograd import no_gradient
+
+                    mean_r, v = no_gradient("loo_marginals", mean_r, ts), no_gradient("loo_marginals", v, ts)
+        if pending is not None and pending.read():
+            return self._loo_missing(xd, marginals, out_origin)
+        if not marginals:
+            lp = lp.reshape(bs + (lp.shape[-1],))
+            return from_dev(lp[..., 0] if lp.shape[-1] == 1 else lp, out_origin)
+        mean = mean_r.transpose(1, 2).reshape(bs + (n, rhs_t.shape[1]))
+        if not self.mean_is_zero:
+            mean = mean + self._mean_dev()
+        mean = mean[..., 0] if mean.shape[-1] == 1 else mean
+        return from_dev(mean, out_origin), from_dev(v.reshape(bs + (n,)), out_origin)
+
+    def _loo_missing(self, xd, marginals, out_origin):
+        avail = ~torch.isnan(xd[:, 0])
+        sub = Normal(self._mean_dev()[avail], M.submatrix(self._var_dev(), avail), origin=self._origin)
+        res = sub._loo(from_dev(xd[avail], out_origin), marginals)
+        if not marginals:
+            return res
+        out = []
+        for t in res:
+            t = to_dev(t, xd.dtype)
+            full = torch.full((xd.shape[0],), float("nan"), dtype=xd.dtype, device=t.device)
+            out.append(from_dev(full.masked_scatter(avail.to(t.device), t), out_origin))
+        return tuple(out)
 
     def entropy(self):
         return self._out((M.logdet(self._var_dev()) + self.dim * (B.log_2_pi + 1)) / 2)

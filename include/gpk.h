@@ -400,6 +400,30 @@ int gpk_loo_finish_f32(const float* c, int64_t c_bstride, const float* alpha, in
                        int64_t ldr, int64_t r_bstride, int64_t n, int32_t k, const float* g, float* mu, float* var,
                        float* lp, float* P, float* q, int32_t batch, void* stream);
 
+/* Multi-fold cross-validation finish (stheno_b200/random.py, Normal.cv_marginals / cv_logpdf) of y ~ N(m, Sigma),
+ * r = y - m, C = Sigma^-1, with the entries in fold order: fold f holds [offsets[f], offsets[f + 1]) (offsets: n_folds + 1
+ * device int64, offsets[n_folds] = n).  Inputs, per entry in fold order: the CV residuals e = C_II^-1 alpha_I
+ * ([batch][k][n], ld lde, batch stride e_bstride), the whitened z = L_I^-1 alpha_I with C_II = L_I L_I^T (ld ldz), the
+ * variances v = diag C_II^-1 ([batch][n]), r ([batch][k][n], ld ldr; read only for mu); per fold ldet = log det C_II
+ * ([batch][n_folds], batch stride ldet_bstride).  Without g (NULL), into contiguous outputs:
+ *   mu[b][c][i] = r_ci - e_ci   (the CV mean of y_ci minus m_i),   var[b][i] = v_i,
+ *   lp[b][c] = sum_f (-1/2 n_f log 2 pi + 1/2 ldet_f - 1/2 |z_cI|^2)
+ * With g ([batch][k], the upstream gradient of lp) it forms the backward weights instead:
+ *   q[b][c][i] = g_c e_ci,   s[b][f] = 1/2 sum_c g_c
+ * so that with P block-diagonal, P_I = s_f C_II^-1 + 1/2 sum_c q_cI e_cI^T, and beta_c = Sigma^-1 q_c:
+ * d(sum_c g_c lp_c)/dSigma = -Sigma^-1 P Sigma^-1 + 1/2 sum_c (beta_c alpha_c^T + alpha_c beta_c^T), d/dr_c = -beta_c.
+ * Every output may be NULL (not formed).  One CTA per column sums lp in a fixed order (the entries, then the folds): the
+ * value is the same bit for bit from run to run.  fp64 arithmetic and sums in both precisions. */
+int gpk_cv_finish_f64(const int64_t* offsets, int32_t n_folds, const double* e, int64_t lde, int64_t e_bstride,
+                      const double* z, int64_t ldz, int64_t z_bstride, const double* v, int64_t v_bstride,
+                      const double* ldet, int64_t ldet_bstride, const double* r, int64_t ldr, int64_t r_bstride, int64_t n,
+                      int32_t k, const double* g, double* mu, double* var, double* lp, double* q, double* s, int32_t batch,
+                      void* stream);
+int gpk_cv_finish_f32(const int64_t* offsets, int32_t n_folds, const float* e, int64_t lde, int64_t e_bstride,
+                      const float* z, int64_t ldz, int64_t z_bstride, const float* v, int64_t v_bstride, const float* ldet,
+                      int64_t ldet_bstride, const float* r, int64_t ldr, int64_t r_bstride, int64_t n, int32_t k,
+                      const float* g, float* mu, float* var, float* lp, float* q, float* s, int32_t batch, void* stream);
+
 /* Measurement helper (bench.py): runs a register-resident fp64 tensor-core (DMMA) loop on every SM and returns the
  * achieved TFLOP/s -- the denominator of the fp64 roofline -- or a negative error code.  Synchronises the device. */
 double gpk_probe_dmma_tflops(void);

@@ -65,6 +65,8 @@ _SIGNATURES = {
     "gpk_feature_eval_bwd": [_ptr, _i64, _i64, _i32, _ptr, _ptr, _ptr, _i64, _ptr, _i64, _i32, _ptr, _i64, _ptr, _i64, _i32,
                              _ptr],
     "gpk_loo_finish": [_ptr, _i64, _ptr, _i64, _i64, _ptr, _i64, _i64, _i64, _i32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr],
+    "gpk_cv_finish": [_ptr, _i32, _ptr, _i64, _i64, _ptr, _i64, _i64, _ptr, _i64, _ptr, _i64, _ptr, _i64, _i64, _i64, _i32, _ptr,
+                      _ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr],
 }
 _PLAIN = {
     "gpk_version": ([], c_int32),

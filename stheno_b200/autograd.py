@@ -17,7 +17,7 @@ import torch
 
 from . import _lib, ops
 
-__all__ = ["kernel_logpdf", "dense_logpdf", "kernel_loo", "dense_loo", "kernel_matrix_grad", "kernel_cross_grad", "kernel_diag_grad", "exact_posterior",
+__all__ = ["kernel_logpdf", "dense_logpdf", "kernel_loo", "dense_loo", "kernel_cv", "dense_cv", "kernel_matrix_grad", "kernel_cross_grad", "kernel_diag_grad", "exact_posterior",
            "sparse_posterior_marginals", "subspace_cov", "no_gradient", "function_sample"]
 
 
@@ -145,6 +145,13 @@ def _loo_G(ch, alpha, c, g):
         ops.gemm_nt(Kinv[b : b + 1] * Pp[b : b + 1], Kinv[b : b + 1], Gm[b : b + 1], alpha=-1.0, beta=0.0, lower=True)
     del Kinv
     beta = ch.full_solve(q)
+    _add_sym_outer(ch, Gm, alpha, beta)
+    return Gm, beta
+
+
+def _add_sym_outer(ch, Gm, alpha, beta):
+    """``Gm += 1/2 sum_c (beta_c alpha_c^T + alpha_c beta_c^T)`` on the lower tiles, then the lower triangle mirrored."""
+    Bn, n, n_pad, k = ch.batch, ch.n, ch.n_pad, alpha.shape[1]
     kp = ops.round_up(2 * k, 16)
     A = torch.zeros(Bn, n_pad, kp, dtype=ch.dtype, device=ch.device)
     Bm = torch.zeros(Bn, n_pad, kp, dtype=ch.dtype, device=ch.device)
@@ -153,7 +160,114 @@ def _loo_G(ch, alpha, c, g):
     for b in range(Bn):
         ops.gemm_nt(A[b : b + 1], Bm[b : b + 1], Gm[b : b + 1], alpha=0.5, beta=1.0, lower=True)
     ops.symmetrize_(Gm, n_pad)
+
+
+# ---- multi-fold cross-validation log densities -------------------------------------------------------------------------------
+#
+# C = K^-1, alpha_c = C r_c, e_cI = C_II^-1 alpha_cI, CV_c = sum_I (-1/2 |I| log 2 pi + 1/2 log det C_II - 1/2 alpha_cI^T e_cI).
+# For L = sum_c g_c CV_c, with q_c = g_c e_c, beta_c = K^-1 q_c and P block-diagonal, P_I = 1/2 sum_c g_c (C_II^-1 + e_cI e_cI^T):
+#   dL/dK   = -K^-1 P K^-1 + 1/2 sum_c (beta_c alpha_c^T + alpha_c beta_c^T)
+#   dL/dr_c = -beta_c
+def _cv_G(ch, folds, g):
+    """``(dL/dK [B, n_pad, n_pad] symmetric, beta [B, k, n])`` (fold order) from the factor, the :class:`ops.CVFolds` of the
+    forward and the upstream ``g [B, k]``.  ``Y = P K^-1`` is formed fold by fold, ``Y[I, :] = P_I K^-1[I, :]``: a product whose
+    contraction runs over a 16-aligned window of ``K^-1``'s columns around ``I`` (``K^-1`` is symmetric), the block ``P_I``
+    embedded at its place in that window.  A fold's GEMM writes ``round_up(n_f)`` rows, reaching into the rows of the folds
+    after it, so every product is added into the zeroed ``Y``: the rows of ``P_I``'s padding are zero and add nothing, in
+    whatever order the folds are visited.  ``K^-1 P K^-1 = Y^T K^-1``.  At most three ``n_pad^2``
+    buffers at once: ``V`` and ``K^-1``; ``K^-1``, ``Y`` and ``Y^T``; ``K^-1``, ``Y^T`` and ``dL/dK``."""
+    Bn, n, n_pad = ch.batch, ch.n, ch.n_pad
+    alpha, off, sizes = folds.alpha, folds.off, folds.sizes
+    k = alpha.shape[1]
+    q, s = ops.cv_finish(folds.offsets, folds.e, g=g.contiguous())
+    Kinv = _inverse_lower(ch, 1.0)
+    ops.symmetrize_(Kinv, n_pad)
+    Y = torch.zeros(Bn, n_pad + ops.TILE, n_pad, dtype=ch.dtype, device=ch.device)
+    kp = ops.round_up(k, 16)
+    for p, (fs, chols, idx) in folds.groups.items():
+        P = torch.cat([_inverse_lower(cg, 1.0) for cg in chols])  # [G B, p, p]: C_II^-1, padded with the identity
+        ops.symmetrize_(P, p)
+        inside = idx.repeat_interleave(Bn, dim=0) >= 0
+        P.masked_fill_(~(inside[:, :, None] & inside[:, None, :]), 0.0)
+        P.mul_(s[:, fs].t().reshape(-1, 1, 1))  # slot i B + b: s[b, fs[i]]
+        A = torch.zeros(P.shape[0], p, kp, dtype=ch.dtype, device=ch.device)
+        Bm = torch.zeros_like(A)
+        A[:, :, :k], Bm[:, :, :k] = folds.to_slots(q, p), folds.to_slots(folds.e, p)
+        ops.gemm_nt(A, Bm, P, alpha=0.5, beta=1.0)
+        for i, f in enumerate(fs):
+            o, nf = off[f], sizes[f]
+            a0 = o // 16 * 16
+            kw = ops.round_up(o + nf - a0, 16)
+            Pe = torch.zeros(Bn, p, kw, dtype=ch.dtype, device=ch.device)
+            Pe[:, :nf, o - a0 : o - a0 + nf] = P[i * Bn : (i + 1) * Bn, :nf, :nf]
+            ops.gemm_nt(Pe, Kinv[:, :, a0 : a0 + kw], Y[:, o : o + p, :], alpha=1.0, beta=1.0)
+    del P
+    Yt = ops.transpose(Y, n_pad, n_pad)  # K^-1 P
+    del Y
+    Gm = torch.empty_like(Kinv)
+    for b in range(Bn):
+        ops.gemm_nt(Yt[b : b + 1], Kinv[b : b + 1], Gm[b : b + 1], alpha=-1.0, beta=0.0, lower=True)
+    del Kinv, Yt
+    beta = ch.full_solve(q)
+    _add_sym_outer(ch, Gm, alpha, beta)
     return Gm, beta
+
+
+class _KernelCV(torch.autograd.Function):
+    """The summed fold log densities ``[B, k]`` of ``N(0, k(x, x) + noise + jitter I)`` at ``rhs_t``, the entries in fold
+    order (``sizes``: the fold sizes); other arguments as :class:`_KernelLogpdf`'s.  The forward runs the launches of the
+    no-grad route (``Chol.cv``)."""
+
+    @staticmethod
+    def forward(ctx, flat, coefs, xg, noise_scalar, noise_vec, rhs_t, jitter, params, sizes):
+        ch = ops.chol_from_kernel(flat, xg.detach().contiguous(), noise_scalar=float(noise_scalar),
+                                  noise_vec=None if noise_vec is None else noise_vec.detach(), jitter=jitter,
+                                  rhs_t=rhs_t.detach(), full_precision=True)
+        _, _, lp, folds = ch.cv(rhs_t.detach(), sizes, want_mean=False)
+        ctx.ch, ctx.flat, ctx.folds = ch, flat, folds
+        ctx.xg = xg.detach().contiguous()
+        ctx.has_nv = noise_vec is not None
+        return lp
+
+    @staticmethod
+    def backward(ctx, g):
+        ch, flat, xg = ctx.ch, ctx.flat, ctx.xg
+        Gm, beta = _cv_G(ch, ctx.folds, g)
+        ps = _param_buf(ctx.needs_input_grad[7], xg.shape[1], xg)
+        term_sum, grad_xg, diag = _bwd_kernel(flat, xg, Gm, ch.n, ps)
+        del Gm
+        grad_coefs = term_sum[:, : len(flat.terms)].sum(0)
+        grad_nv = diag if ctx.has_nv else None
+        return None, grad_coefs, grad_xg, diag.sum(), grad_nv, -beta, None, _param_grad(flat, ps), None
+
+
+def kernel_cv(flat, xg, noise_scalar, noise_vec, rhs_t, jitter, sizes):
+    """Differentiable summed fold log densities ``[B, k]`` of entries in fold order (``sizes``: the fold sizes); arguments
+    and gradients as :func:`kernel_logpdf`'s."""
+    return _KernelCV.apply(flat, coef_tensor(flat, xg), xg, _scalar(noise_scalar, xg), noise_vec, rhs_t, jitter,
+                           param_tensor(flat, xg), tuple(sizes))
+
+
+class _DenseCV(torch.autograd.Function):
+    """:class:`_KernelCV` for an explicit dense ``K [B, n, n]`` (+ ``jitter I``), with a gradient w.r.t. ``K`` itself."""
+
+    @staticmethod
+    def forward(ctx, K, rhs_t, jitter, sizes):
+        ch = ops.chol_from_dense(K.detach(), jitter=jitter, rhs_t=rhs_t.detach())
+        _, _, lp, folds = ch.cv(rhs_t.detach(), sizes, want_mean=False)
+        ctx.ch, ctx.folds = ch, folds
+        return lp
+
+    @staticmethod
+    def backward(ctx, g):
+        ch = ctx.ch
+        Gm, beta = _cv_G(ch, ctx.folds, g)
+        n = ch.n
+        return Gm[:, :n, :n].contiguous(), -beta, None, None
+
+
+def dense_cv(K, rhs_t, jitter, sizes):
+    return _DenseCV.apply(K, rhs_t, jitter, tuple(sizes))
 
 
 class _KernelLoo(torch.autograd.Function):

@@ -236,6 +236,19 @@ class KernelDense(Dense):
                                     noise_vec=None if self.noise_vec is None else self.noise_vec.detach(), jitter=_B.epsilon,
                                     rhs_t=rhs_t, full_precision=True)
 
+    def permuted(self, perm):
+        """The same covariance with its entries reordered by the device index ``perm``: K1 evaluates at ``x[perm]``, so no
+        ``n^2`` permutation is copied; gradients reach ``xg`` and the noise vector through the gather."""
+        nv = None if self.noise_vec is None else self.noise_vec[..., perm]
+        return KernelDense(self.flat, self.xg[:, :, perm], self.batch_shape, self.noise_scalar, nv, self.origin, self.noise_t)
+
+    def cv_grad(self, rhs_t, sizes):
+        """Differentiable summed fold log densities ``[B, k]`` of entries in fold order (``sizes``: the fold sizes), with the
+        gradients of :meth:`logpdf_grad`."""
+        from .autograd import kernel_cv
+
+        return kernel_cv(self.flat, self.xg, self.noise, self.noise_vec, rhs_t, _B.epsilon, sizes)
+
     def loo_grad(self, rhs_t):
         """Differentiable summed leave-one-out log densities ``[B, k]``, with the gradients of :meth:`logpdf_grad`."""
         from .autograd import kernel_loo

@@ -501,6 +501,21 @@ class Chol:
         mean, var, lp = loo_finish(c, alpha, r, want_mean=want_mean)
         return mean, var, lp, alpha, c
 
+    def cv(self, r, sizes, want_mean=True, chunk=2048):
+        """Multi-fold cross-validation quantities of ``N(0, L L^T)`` at the fused right-hand sides ``r [B, k, n]``, the
+        entries in fold order (fold ``f`` is the ``sizes[f]`` entries after the folds before it).  With ``C = (L L^T)^-1``
+        and ``alpha = C r``: ``(mean [B, k, n] (the CV mean minus the prior mean; None without want_mean), var [B, n],
+        lp [B, k], folds)`` where ``folds`` (:class:`CVFolds`) holds ``alpha``, the residuals ``e`` and the factors of
+        the blocks ``C_II`` for the backward (:func:`cv_finish`)."""
+        k, n = self.k, self.n
+        arows = self.new_rows(k)
+        arows[:, :k, :n] = self.rhs_half()
+        self.solve_rows_t_(arows)
+        alpha = arows[:, :k, :n]
+        folds = CVFolds(self, sizes, alpha, chunk)
+        mean, var, lp = cv_finish(folds.offsets, folds.e, folds.z, folds.v, folds.ldet, r, want_mean=want_mean)
+        return mean, var, lp, folds
+
     def half_solve(self, bt):
         """``bt [B, m, n]`` (rows = right-hand sides) -> ``(L^-1 b)^T [B, m, n]``."""
         m = bt.shape[1]
@@ -549,6 +564,177 @@ def loo_finish(c, alpha, r=None, g=None, *, want_mean=True, want_var=True, want_
         r.stride(0) if r is not None else 0, n, k, _ptr(g), *[_ptr(t) for t in outs], Bn, _stream(),
     )
     check(rc, "gpk_loo_finish")
+    return outs[3:] if g is not None else outs[:3]
+
+
+#: the batched factorisation launches one grid row per matrix: at most this many fold blocks per call
+_MAX_FOLD_BATCH = 32768
+
+
+class CVFolds:
+    """The diagonal blocks ``C_II`` of ``C = (L L^T)^-1`` for consecutive folds of ``sizes`` entries, factorised, with
+    ``alpha [B, k, n]`` (``C r``) as their right-hand sides.
+
+    Rows of ``V = L^-T`` (``C = V V^T``) from a 128-aligned ``a`` need only the trailing factor ``L[a:, a:]``: identity rows
+    are solved in chunks whose boundaries fall on fold boundaries (at least as tall as the largest fold they hold; one
+    ``[B, rows, n_pad]`` buffer), and each fold's block ``V_I V_I^T`` is formed by the lower-tile GEMM straight into a
+    workspace padded with the identity to ``p = round_up(n_f)``, ``alpha_I`` in its right-hand-side rows -- consecutive
+    folds of one size in one batched GEMM.  Folds of one padded size are factorised as one batch: ``log det C_II``,
+    ``z_I = L_I^-1 alpha_I``, the residuals ``e_I = C_II^-1 alpha_I`` and ``diag C_II^-1``.  Attributes (fold order):
+    ``offsets`` (device int64 ``[F + 1]``), ``alpha``, ``e``, ``z`` ``[B, k, n]``, ``v [B, n]``, ``ldet [B, F]``; ``groups``:
+    ``{p: (folds, [Chol of <= _MAX_FOLD_BATCH slots], idx)}`` with slot ``i * B + b`` = fold ``folds[i]``, problem ``b``, and
+    ``idx [len(folds), p]`` the entry of each padded row (-1: padding)."""
+
+    def __init__(self, ch, sizes, alpha, chunk=2048):
+        self.sizes = [int(s) for s in sizes]
+        off = [0]
+        for s in self.sizes:
+            off.append(off[-1] + s)
+        if off[-1] != ch.n or min(self.sizes) < 1:
+            raise ValueError("CVFolds: the fold sizes must be positive and add up to n")
+        self.off, self.alpha, self.batch, self.n = off, alpha, ch.batch, ch.n
+        self.offsets = torch.tensor(off, dtype=torch.int64, device=ch.device)
+        self.pads = [round_up(s) for s in self.sizes]
+        self.members = {}  # padded size -> its folds, in fold order
+        for f, p in enumerate(self.pads):
+            self.members.setdefault(p, []).append(f)
+        self.factor(self.blocks(ch, chunk))
+
+    def blocks(self, ch, chunk=2048):
+        """The fold-block product: ``{p: W [G B, p + round_up(k), p]}``, the blocks ``C_II`` on the lower tiles of each slot
+        (the padding not yet the identity) and ``alpha_I`` in its right-hand-side rows."""
+        Bn, n_pad, off, sizes, pads = ch.batch, ch.n_pad, self.off, self.sizes, self.pads
+        alpha = self.alpha
+        k = alpha.shape[1]
+        dev, dt = ch.device, ch.dtype
+        F = len(sizes)
+        slot, Ws, self.idxs = {}, {}, {}
+        a_ext = torch.cat([alpha, torch.zeros(Bn, k, 1, dtype=dt, device=dev)], dim=2)  # entry -1 (padding) reads 0
+        for p, fs in self.members.items():
+            for i, f in enumerate(fs):
+                slot[f] = i
+            ar = torch.arange(p)
+            nf = torch.tensor([sizes[f] for f in fs])
+            idx = torch.where(ar[None, :] < nf[:, None], torch.tensor([off[f] for f in fs])[:, None] + ar[None, :], -1)
+            self.idxs[p] = idx = idx.to(dev)
+            W = torch.zeros(len(fs) * Bn, p + round_up(k), p, dtype=dt, device=dev)
+            W[:, p : p + k, :] = a_ext[:, :, idx].permute(2, 0, 1, 3).reshape(len(fs) * Bn, k, p)
+            Ws[p] = W
+        plan, f = [], 0
+        while f < F:
+            a = off[f] // TILE * TILE
+            g = f + 1
+            while g < F and round_up(off[g + 1] - a) <= chunk:
+                g += 1
+            plan.append((a, f, g))
+            f = g
+        rows_max = max(round_up(off[g] - a) for a, _, g in plan) + TILE  # a fold's p rows from its start stay inside
+        buf = torch.empty(Bn, rows_max, n_pad, dtype=dt, device=dev)
+        fn = _fn("gpk_trsm_right", dt)
+        Lp = ch.L_padded()
+        for a, f0, f1 in plan:
+            rows, m = round_up(off[f1] - a), n_pad - a
+            X = buf[:, :, :m]
+            X.zero_()
+            X[:, :rows].diagonal(dim1=1, dim2=2).fill_(1.0)
+            L = Lp[:, a:, a:]
+            em = _emulation(dt, dev, lambda lib, s: lib.gpk_trsm_right_oz_ws_bytes(m, rows, s) if Bn == 1 else 0)
+            rc = fn(_ptr(L), L.stride(1), L.stride(0), m, _ptr(X), X.stride(1), X.stride(0), rows, Bn, *em, _stream())
+            check(rc, "gpk_trsm_right")
+            i = f0
+            while i < f1:  # runs of consecutive folds of one size: consecutive slots of one group
+                j = i + 1
+                while j < f1 and sizes[j] == sizes[i]:
+                    j += 1
+                nf, p, s0 = sizes[i], pads[i], slot[i]
+                W = Ws[p]
+                for b in range(Bn):  # fold t of the run: rows [off[i] + t nf - a, + p) of the chunk, slot (s0 + t) B + b
+                    A = buf.as_strided((j - i, p, m), (nf * buf.stride(1), buf.stride(1), 1),
+                                       b * buf.stride(0) + (off[i] - a) * buf.stride(1))
+                    C = W.as_strided((j - i, p, p), (Bn * W.stride(0), W.stride(1), 1), (s0 * Bn + b) * W.stride(0))
+                    gemm_nt(A, A, C, alpha=1.0, beta=0.0, lower=True)
+                i = j
+        return Ws
+
+    def factor(self, Ws):
+        """The fold factorisations, in place on the workspaces of :meth:`blocks`: the padding of each block back to the
+        identity, then one batched factorisation per padded size and its solves; sets ``e``, ``z``, ``v``, ``ldet``,
+        ``groups``."""
+        Bn, n, k = self.batch, self.n, self.alpha.shape[1]
+        dev, dt = self.alpha.device, self.alpha.dtype
+        self.e = torch.zeros(Bn, k, n, dtype=dt, device=dev)
+        self.z = torch.zeros(Bn, k, n, dtype=dt, device=dev)
+        self.v = torch.empty(Bn, n, dtype=dt, device=dev)
+        self.ldet = torch.empty(Bn, len(self.sizes), dtype=dt, device=dev)
+        self.groups = {}
+        for p, fs in self.members.items():
+            W, idx = Ws.pop(p), self.idxs[p]
+            G = len(fs)
+            if any(self.sizes[f] < p for f in fs):
+                nf = torch.tensor([self.sizes[f] for f in fs], device=dev).repeat_interleave(Bn)
+                inside = torch.arange(p, device=dev)[None, :] < nf[:, None]
+                W[:, :p, :].masked_fill_(~(inside[:, :, None] & inside[:, None, :]), 0.0)
+                W[:, :p, :].diagonal(dim1=1, dim2=2).masked_fill_(~inside, 1.0)
+            chols, es, zs, vs, lds = [], [], [], [], []
+            for s0 in range(0, G * Bn, _MAX_FOLD_BATCH):
+                cg = _potrf(W[s0 : s0 + _MAX_FOLD_BATCH], p, p, W.shape[1] - p, k)
+                er = cg.new_rows(k)
+                er[:, :k] = cg.rhs_half()
+                cg.solve_rows_t_(er)
+                chols.append(cg)
+                es.append(er[:, :k])
+                zs.append(cg.rhs_half())
+                vs.append(cg.inverse_diag())
+                lds.append(cg.logdet)
+            self.groups[p] = (fs, chols, idx)
+            pos = idx.reshape(-1)
+            inside = pos >= 0
+            pos = pos[inside]
+            for dst, parts in ((self.e, es), (self.z, zs)):
+                t = torch.cat(parts).reshape(G, Bn, k, p).permute(1, 2, 0, 3).reshape(Bn, k, G * p)
+                dst[:, :, pos] = t[:, :, inside]
+            t = torch.cat(vs).reshape(G, Bn, p).permute(1, 0, 2).reshape(Bn, G * p)
+            self.v[:, pos] = t[:, inside]
+            self.ldet[:, fs] = torch.cat(lds).reshape(G, Bn).t()
+
+    def to_slots(self, t, p):
+        """Entries ``t [B, c, n]`` (fold order) -> the padded rows of group ``p``'s slots ``[G B, p, c]`` (padding 0)."""
+        fs, _, idx = self.groups[p]
+        Bn, c = t.shape[0], t.shape[1]
+        t_ext = torch.cat([t, torch.zeros(Bn, c, 1, dtype=t.dtype, device=t.device)], dim=2)
+        return t_ext[:, :, idx].permute(2, 0, 3, 1).reshape(len(fs) * Bn, idx.shape[1], c)
+
+
+def cv_finish(offsets, e, z=None, v=None, ldet=None, r=None, g=None, *, want_mean=True, want_var=True, want_lp=True):
+    """``gpk_cv_finish`` on entries in fold order (fold ``f`` = ``[offsets[f], offsets[f + 1])``, ``offsets`` a device
+    int64 ``[F + 1]``): the residuals ``e [B, k, n]`` (``C_II^-1 alpha_I``), ``z [B, k, n]`` (``L_I^-1 alpha_I``), ``v [B, n]``
+    (``diag C_II^-1``), ``ldet [B, F]`` (``log det C_II``) and ``r [B, k, n]``.  Without ``g``: ``(mean [B, k, n], var [B, n],
+    lp [B, k])`` with ``mean = r - e``, ``var = v`` and ``lp`` the summed fold log densities (None for those not wanted).
+    With the upstream gradient ``g [B, k]`` of ``lp``: the backward weights ``(q [B, k, n], s [B, F])``, ``q = g e``,
+    ``s = 1/2 sum_c g_c``."""
+    _require_cuda(offsets, e, z, v, ldet, r, g)
+    Bn, k, n = e.shape
+    F = offsets.shape[0] - 1
+    for t, shape in ((z, (Bn, k, n)), (r, (Bn, k, n)), (v, (Bn, n)), (ldet, (Bn, F)), (g, (Bn, k))):
+        if t is not None and tuple(t.shape) != shape:
+            raise ValueError("cv_finish: shapes do not match")
+    e, z, v, ldet, r = [None if t is None else (t if t.stride(-1) == 1 else t.contiguous()) for t in (e, z, v, ldet, r)]
+    new = lambda *shape: torch.empty(*shape, device=e.device, dtype=e.dtype)  # noqa: E731
+    if g is not None:
+        outs = (None, None, None, new(Bn, k, n), new(Bn, F))
+        g = g.contiguous()
+    else:
+        if want_mean and r is None:
+            raise ValueError("cv_finish: the mean needs r")
+        outs = (new(Bn, k, n) if want_mean else None, new(Bn, n) if want_var else None, new(Bn, k) if want_lp else None,
+                None, None)
+    ld = lambda t: (t.stride(1) if k > 1 else n) if t is not None else 0  # noqa: E731
+    bs = lambda t: t.stride(0) if t is not None else 0  # noqa: E731
+    rc = _fn("gpk_cv_finish", e.dtype)(
+        _ptr(offsets), F, _ptr(e), ld(e), bs(e), _ptr(z), ld(z), bs(z), _ptr(v), bs(v), _ptr(ldet), bs(ldet), _ptr(r), ld(r),
+        bs(r), n, k, _ptr(g), *[_ptr(t) for t in outs], Bn, _stream(),
+    )
+    check(rc, "gpk_cv_finish")
     return outs[3:] if g is not None else outs[:3]
 
 

@@ -79,6 +79,14 @@ def _loo_structured(var, rhs_t):
     if isinstance(var, M.Diagonal):
         d = var.diag.reshape(-1, n)
         return 1.0 / d, rhs_t / d.unsqueeze(1)
+    d3, H, alpha = _woodbury_inverse(var, rhs_t)
+    return 1.0 / d3 - (H * H).sum(1), alpha
+
+
+def _woodbury_inverse(var, rhs_t):
+    """``(d [B, n], H [B, r, n], alpha [B, k, n])`` of a Woodbury covariance ``D + U U^T``: ``Sigma^-1 = D^-1 - H^T H`` with
+    ``H = L^-1 U^T D^-1`` (``L L^T`` the Schur complement, regularised by ``B.epsilon``) and ``alpha = Sigma^-1 r``."""
+    n = rhs_t.shape[-1]
     U, d = var.lr.left, var.diag_m.diag
     U3 = U.reshape((-1,) + tuple(U.shape[-2:]))
     r = U3.shape[-1]
@@ -87,10 +95,52 @@ def _loo_structured(var, rhs_t):
     S = torch.eye(r, dtype=U.dtype, device=U.device) + U3.transpose(1, 2) @ Ud
     L = torch.linalg.cholesky(S + B.epsilon * torch.eye(r, dtype=U.dtype, device=U.device))
     H = torch.linalg.solve_triangular(L, Ud.transpose(1, 2), upper=False)  # [B, r, n]: L^-1 U^T D^-1
-    c = 1.0 / d3 - (H * H).sum(1)
     h = H @ rhs_t.transpose(1, 2)  # [B, r, k]
     alpha = rhs_t / d3.unsqueeze(1) - (H.transpose(1, 2) @ h).transpose(1, 2)
-    return c, alpha
+    return d3, H, alpha
+
+
+def _fold_order(folds, n):
+    """``(perm [n] int64, sizes)`` of fold labels: the stable sort of the labels and the sizes of the folds in label order.
+    Raises ``ValueError`` unless ``folds`` is a 1-D array or tensor of ``n`` finite integer labels."""
+    lab = folds.detach().cpu().numpy() if isinstance(folds, torch.Tensor) else np.asarray(folds)
+    if lab.ndim != 1 or lab.shape[0] != n:
+        raise ValueError(f"folds must be a 1-D array of {n} labels, got shape {lab.shape}")
+    if lab.dtype.kind == "f":
+        if not np.isfinite(lab).all() or (lab != np.round(lab)).any():
+            raise ValueError("fold labels must be finite integers")
+        lab = lab.astype(np.int64)
+    elif lab.dtype.kind not in "iu":
+        raise ValueError(f"fold labels must be integers, got dtype {lab.dtype}")
+    perm = np.argsort(lab, kind="stable")
+    sizes = np.unique(lab[perm], return_counts=True)[1]
+    return perm, [int(s) for s in sizes]
+
+
+def _cv_woodbury(var, rhs_t, sizes):
+    """``(mean [B, k, n], var [B, n], lp [B, k])`` of a Woodbury covariance whose entries are in fold order, in differentiable
+    torch ops: the fold blocks of ``Sigma^-1`` by the inversion lemma, ``D_I^-1 - H_I^T H_I`` (``O(sum n_f^2 r)``), factorised
+    in one batch per fold size."""
+    d3, H, alpha = _woodbury_inverse(var, rhs_t)
+    Bn, k, n = rhs_t.shape
+    off = np.concatenate([[0], np.cumsum(sizes)])
+    pos, means, vs, lp = [], [], [], 0.0
+    for s in sorted(set(sizes)):
+        starts = off[:-1][np.asarray(sizes) == s]
+        idx = torch.as_tensor(starts[:, None] + np.arange(s)[None, :], device=rhs_t.device)  # [G, s]
+        HI = H[:, :, idx].permute(0, 2, 1, 3)  # [B, G, r, s]
+        C = torch.diag_embed(1.0 / d3[:, idx]) - HI.transpose(-1, -2) @ HI
+        Lc = torch.linalg.cholesky(C)
+        aI = alpha[:, :, idx].permute(0, 2, 3, 1)  # [B, G, s, k]
+        z = torch.linalg.solve_triangular(Lc, aI, upper=False)
+        e = torch.linalg.solve_triangular(Lc.transpose(-1, -2), z, upper=True)
+        ldet = 2 * torch.log(torch.diagonal(Lc, dim1=-2, dim2=-1)).sum(-1)  # [B, G]
+        lp = lp + 0.5 * ((ldet.sum(1) - len(starts) * s * B.log_2_pi).unsqueeze(-1) - (z * z).sum((1, 2)))
+        pos.append(idx.reshape(-1))
+        means.append((rhs_t[:, :, idx] - e.permute(0, 3, 1, 2)).reshape(Bn, k, -1))
+        vs.append(torch.diagonal(torch.cholesky_inverse(Lc), dim1=-2, dim2=-1).reshape(Bn, -1))
+    order = torch.argsort(torch.cat(pos))
+    return torch.cat(means, -1)[:, :, order], torch.cat(vs, -1)[:, order], lp
 
 
 def _loo_torch(c, alpha, r):
@@ -379,6 +429,108 @@ class Normal(RandomVector):
         avail = ~torch.isnan(xd[:, 0])
         sub = Normal(self._mean_dev()[avail], M.submatrix(self._var_dev(), avail), origin=self._origin)
         res = sub._loo(from_dev(xd[avail], out_origin), marginals)
+        if not marginals:
+            return res
+        out = []
+        for t in res:
+            t = to_dev(t, xd.dtype)
+            full = torch.full((xd.shape[0],), float("nan"), dtype=xd.dtype, device=t.device)
+            out.append(from_dev(full.masked_scatter(avail.to(t.device), t), out_origin))
+        return tuple(out)
+
+    # ---- multi-fold cross-validation (blocked / grouped / K-fold) ----------------------------------------------------------
+    def cv_marginals(self, x, folds):
+        """Mean and variance of every ``x_i`` given all the entries outside its fold, with the shapes of
+        :meth:`loo_marginals`.  ``folds``: ``n`` integer labels (array or tensor; any values, in any order); entries with
+        one label form a fold, and one ``folds`` serves every batch member and column.  NaN entries of a single column are
+        missing: dropped before folding, with NaN marginals.  With ``Sigma = var + B.epsilon I``, ``C = Sigma^-1``,
+        ``alpha = C (x - mean)`` and ``C_II`` the block of fold ``I``: mean ``x_I - C_II^-1 alpha_I``, variance
+        ``diag C_II^-1``.  Singleton folds give :meth:`loo_marginals`, a single fold the prior marginals.  Gradients flow
+        through diagonal and Woodbury covariances only; elsewhere a backward through these values raises."""
+        return self._cv(x, folds, marginals=True)
+
+    def cv_logpdf(self, x, folds):
+        """``sum_I log p(x_I | x_-I)`` over the folds of ``folds`` (as in :meth:`cv_marginals`), with the output shapes of
+        :meth:`logpdf` and its missing-data rule; a fold whose entries are all missing contributes nothing.  Singleton
+        folds give :meth:`loo_logpdf`, a single fold :meth:`logpdf`.  Differentiable on every route, the kernel-matrix
+        one with an analytic gradient on the GPU."""
+        return self._cv(x, folds, marginals=False)
+
+    def _cv(self, x, folds, marginals):
+        out_origin = origin_of(x) if self._origin is None else self._origin
+        var = self._var_dev()
+        xd = uprank(to_dev(x, None)).to(var.dtype)
+        n = var.shape[-1]
+        perm, sizes = _fold_order(folds, n)
+        if max(sizes, default=1) == 1:  # singleton folds are leave-one-out, without a 128-padded workspace per entry
+            return self._loo(x, marginals)
+        pending = None
+        if xd.dim() == 2 and xd.shape[1] == 1:  # missing data, detected as in logpdf
+            if isinstance(x, torch.Tensor) and x.is_cuda:
+                if _allow_missing:
+                    pending = _NanFlag(xd)
+            else:
+                host = x.detach().numpy() if isinstance(x, torch.Tensor) else np.asarray(x, dtype=float)
+                if np.isnan(host).any():
+                    return self._cv_missing(xd, folds, marginals, out_origin)
+        diff = xd if self.mean_is_zero else xd - self._mean_dev()
+        d3, bs = batch_flatten(diff, 2)
+        rhs_t = d3.transpose(1, 2).contiguous()  # [B, k, n]
+        p = torch.as_tensor(perm, device=rhs_t.device)
+        rhs_p = rhs_t[:, :, p]  # fold order: fold f is one contiguous range of entries
+        if isinstance(var, M.Diagonal):  # the folds decouple into single entries: leave-one-out
+            c, alpha = _loo_structured(var, rhs_t)
+            mean_r, v, lp = _loo_torch(c, alpha, rhs_t)
+            p = None
+        elif isinstance(var, M.Woodbury):
+            vp = M.Woodbury(M.Diagonal(var.diag_m.diag[..., p], var.origin), M.LowRank(var.lr.left[..., p, :], var.origin))
+            mean_r, v, lp = _cv_woodbury(vp, rhs_p, sizes)
+        else:
+            if isinstance(var, M.LowRank):
+                var = M.Dense(var.dev, var.origin)
+            ts = _grad_tensors(var, rhs_t)
+            mean_r = v = None
+            if isinstance(var, M.KernelDense):
+                vp = var.permuted(p)
+                if ts and not marginals:
+                    lp = vp.cv_grad(rhs_p, sizes)
+                else:
+                    ch = vp.loo_chol(rhs_p.detach())
+            elif ts and not marginals:
+                from .autograd import dense_cv
+
+                K3, _ = batch_flatten(var.dev, 2)
+                lp = dense_cv(K3[:, p][:, :, p], rhs_p, B.epsilon, sizes)  # gradient w.r.t. the assembled covariance
+            else:
+                K3, _ = batch_flatten(var.dev, 2)
+                ch = ops.chol_from_dense(K3.detach()[:, p][:, :, p], jitter=B.epsilon, rhs_t=rhs_p.detach())
+            if marginals or not ts:
+                mean_r, v, lp, _ = ch.cv(rhs_p.detach(), sizes, want_mean=marginals)
+                del ch
+                if ts:  # raw-pointer values: a gradient through them would be silently wrong
+                    from .autograd import no_gradient
+
+                    mean_r, v = no_gradient("cv_marginals", mean_r, ts), no_gradient("cv_marginals", v, ts)
+        if pending is not None and pending.read():
+            return self._cv_missing(xd, folds, marginals, out_origin)
+        if not marginals:
+            lp = lp.reshape(bs + (lp.shape[-1],))
+            return from_dev(lp[..., 0] if lp.shape[-1] == 1 else lp, out_origin)
+        if p is not None:  # back to the caller's order
+            inv = torch.empty_like(p)
+            inv[p] = torch.arange(n, device=p.device)
+            mean_r, v = mean_r[:, :, inv], v[:, inv]
+        mean = mean_r.transpose(1, 2).reshape(bs + (n, rhs_t.shape[1]))
+        if not self.mean_is_zero:
+            mean = mean + self._mean_dev()
+        mean = mean[..., 0] if mean.shape[-1] == 1 else mean
+        return from_dev(mean, out_origin), from_dev(v.reshape(bs + (n,)), out_origin)
+
+    def _cv_missing(self, xd, folds, marginals, out_origin):
+        avail = ~torch.isnan(xd[:, 0])
+        lab = folds.detach().cpu() if isinstance(folds, torch.Tensor) else torch.as_tensor(np.asarray(folds))
+        sub = Normal(self._mean_dev()[avail], M.submatrix(self._var_dev(), avail), origin=self._origin)
+        res = sub._cv(from_dev(xd[avail], out_origin), lab[avail.cpu()], marginals)
         if not marginals:
             return res
         out = []
